@@ -6,7 +6,7 @@
     python bench.py --impl reference --steps 5 --warmup 1          # the reference's CPU path (oracle port; Ceres itself is not installable)
 
 Workload (config.workload): BASELINE.json configs[2] -- ONE synthetic problem of 100 cameras / 200k points / 1.6M observations.
-`--gpus N` is STRONG scaling, as BASELINE.json states it ("1/2/4/8 x B200 NCCL-reduced camera system"): the 200k points are
+`--gpus N` is STRONG scaling, as BASELINE.json states it ("1/2/4/8 x H100 NCCL-reduced camera system"): the 200k points are
 sharded over the N ranks, the 100 cameras are replicated, the reduced camera system is summed over ranks once per LM iteration.
 (Weak scaling -- 200k points per rank -- is measured too and reported under the key "weak".)  `--workload cfg2` selects
 configs[1] (20 / 10k / 80k).
@@ -40,7 +40,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 (not measured)"
 
 
 def algorithmic_bytes(nc, npts, nobs):
@@ -213,6 +213,16 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, prob, summary):
+    """What a caller of the timed path receives after its last LM iteration, as float64 .npy files: the cameras
+    (angle-axis + translation), the points and the shared focal length of this rank's problem, and the final cost.
+    cfg3 writes ~5 MB (200k points x 3 x 8 B)."""
+    cams, pts, focal = prob.download()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in (("cams", cams), ("pts", pts), ("focal", np.array([focal])), ("final_cost", np.array([summary["final_cost"]]))):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, np.float64))
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 def run_ours(args):
     import torch
@@ -263,7 +273,7 @@ def run_ours(args):
         run_steps(prob, capi, args.warmup, profile=1, l2_flush_mb=L2_FLUSH_MB)
     prob.reset()
     with torch.cuda.stream(stream):
-        flush.zero_()                                   # L2 flush before the timed region (inputs < L2 on one GPU)
+        flush.zero_()                                   # L2 flush before the timed region
     barrier()
     launches0 = ctx.kernel_launches
     e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
@@ -279,6 +289,8 @@ def run_ours(args):
     flush_ms = float(s["flush_ms_total"])
     dev_ms = dev_ms_raw - flush_ms
     launches = ctx.kernel_launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, prob, s)
     # Clocks and throttle reasons: NVML / nvidia-smi queries hold the driver lock for 1-40 ms on these hosts and stall the
     # kernel launches of the process they observe (measured: the 0.83 ms step became 1.2-2.2 ms, a 2-GPU step 10 ms), so the
     # sampler does not run inside the reported pass.  It runs during an IDENTICAL second pass of the same K iterations right
@@ -408,7 +420,7 @@ def run_ours(args):
     try:
         fp64_peak = float(json.load(open(os.path.join(ROOT, "profiles", "fp64_peak.json")))["dmma_m8n8k4_tflops"]); fp64_src = "measured (profiles/fp64_peak.json, mma.sync m8n8k4 f64)"
     except Exception:
-        fp64_peak, fp64_src = 40.0, "nominal B200 fp64"
+        fp64_peak, fp64_src = 67.0, "H100 SXM data sheet fp64 tensor (not measured)"
     fp64 = {"flops_per_step": flops_iter, "pair_entries": pair_entries, "peak_tflops": fp64_peak, "peak_source": fp64_src}
     dominant = max(kernels, key=kernels.get)
 
@@ -425,7 +437,7 @@ def run_ours(args):
                                    + (f"; the {args.steps} timed iterations are solves of {SOLVE_ITERS} restarted from x0" if args.steps > SOLVE_ITERS + 4 else ""),
                            "parallelism": f"the problem's points sharded over {world} GPU(s) (strong scaling), cameras replicated, reduced camera system "
                                           f"summed over ranks ({exchange}); every rank factors the 601x601 reduced system redundantly",
-                           "l2": f"flushed: a {L2_FLUSH_MB} MB scratch buffer is written before every timed LM iteration (per-GPU working set ~90 MB < L2); "
+                           "l2": f"flushed: a {L2_FLUSH_MB} MB scratch buffer is written before every timed LM iteration (part of the ~90 MB per-GPU working set would otherwise stay in the 50 MB L2); "
                                  "the flush writes run inside the event bracket and their own event time is subtracted (ms_per_step_incl_flush keeps the raw bracket)"},
                 "wall_ms_per_step": wall_ms / iters, "ms_per_step_incl_flush": dev_ms_raw / iters,
                 "dense_solve_ms": s["solve_ms_total"] / max(1, s["num_linear_solves"]),
@@ -554,7 +566,11 @@ def main():
     ap.add_argument("--workload", default="cfg3", choices=["cfg3", "cfg2"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-stages", action="store_true", help="skip the secondary stage measurements (cfg1 replay)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the cameras, points, focal length and cost after the last timed LM iteration as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

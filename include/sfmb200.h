@@ -1,5 +1,5 @@
 /*
- * sfmb200.h -- C ABI of the B200-native SfM hot path (libsfmb200.so).
+ * sfmb200.h -- C ABI of the H100-native SfM hot path (libsfmb200.so).
  *
  * Drop-in boundary for the three compute stages of royshil/SfM-Toy-Library (SURVEY.md section 8b).
  * Plain pointers and sizes only; the caller owns every host buffer, the library owns device scratch
@@ -53,7 +53,7 @@ int64_t sfmb200_kernel_launches(const sfmb200_ctx* ctx);    /* number of kernels
  * Pass ratio = (double)0.8f to reproduce NN_MATCH_RATIO (SfM2DFeatureUtilities.cpp:35).
  * q [nq*desc_bytes], t [nt*desc_bytes] row-major PACKED bytes (ORB: desc_bytes = 32); 1 <= desc_bytes <= 128.  The kernels are
  * instantiated for 16/32/64/128 bytes; any other width is zero-padded to the next one (every distance unchanged).
- * 32-byte descriptors run on the tcgen05 tensor-core kernel, the other widths on the XOR/POPC kernel.
+ * 32-byte descriptors run on the wgmma tensor-core kernel, the other widths on the XOR/POPC kernel.
  * out_q/out_t/out_d must hold nq entries; *out_n receives the number of survivors (imgIdx is always 0).
  * nt < 2 (undefined behaviour in the reference) yields *out_n = 0.
  * The reference calls this once per image pair with the same images again and again (SfM.cpp:166-206): uploaded images
@@ -66,7 +66,7 @@ int sfmb200_match_knn2_ratio(sfmb200_ctx* ctx, const uint8_t* q, int nq, const u
 /* L2 variant (cv::BFMatcher(NORM_L2), BASELINE.json configs[3] wording "SIFT-128"; the legacy tree's own L2 knn + ratio test is
  * legacy/SfMToyLib_Old/GPUSURFFeatureMatcher.cpp:100-124): float descriptors [n*dim], distance = sqrtf(sum of squared
  * differences).  Integer-valued descriptors in [0, 255] with dim <= 128 (what cv::SIFT produces) are matched EXACTLY as a
- * u8 x u8 -> s32 GEMM on the tcgen05 tensor cores (|a-b|^2 = |a|^2 + |b|^2 - 2<a,b>, every term an exact integer < 2^24, so the
+ * u8 x u8 -> s32 GEMM on the wgmma tensor cores (|a-b|^2 = |a|^2 + |b|^2 - 2<a,b>, every term an exact integer < 2^24, so the
  * float32 sum cv::batchDistance forms is reproduced bit for bit); anything else runs the fp32 SIMT kernel. */
 int sfmb200_match_knn2_ratio_l2(sfmb200_ctx* ctx, const float* q, int nq, const float* t, int nt, int dim,
                                 double ratio, int32_t* out_q, int32_t* out_t, float* out_d, int* out_n);

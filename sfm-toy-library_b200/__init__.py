@@ -1,4 +1,4 @@
-"""sfm-toy-library_b200: B200-native hot path of royshil/SfM-Toy-Library.
+"""sfm-toy-library_b200: H100-native hot path of royshil/SfM-Toy-Library.
 
 The product is the C-ABI shared library built from csrc/ (include/sfmb200.h); this Python package is the thin
 host-side mirror of the reference's stage interface (stages.py), the ctypes binding (capi.py), the multi-GPU

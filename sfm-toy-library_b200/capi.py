@@ -53,7 +53,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise SfmB200Error(f"{LIB_PATH} not found: run `python sfm-toy-library_b200/build.py` (nvcc, sm_100a). There is no CPU fallback.")
+            raise SfmB200Error(f"{LIB_PATH} not found: run `python sfm-toy-library_b200/build.py` (nvcc, sm_90a). There is no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         L.sfmb200_last_error.restype = C.c_char_p
         L.sfmb200_last_error.argtypes = [C.c_void_p]

@@ -5,7 +5,7 @@
 // :158-164, :171-179).  Ceres' algorithm is restated (SURVEY.md appendix A.3): Jacobi column scaling fixed at x0,
 // LM diagonal clamp(diag(J^T J), 1e-6, 1e32)/radius, step-quality radius update, the four termination tests.
 //
-// Design (B200-first, not a Ceres translation):
+// Design (GPU-first, not a Ceres translation):
 //   * The Jacobian is never materialised.  Every pass re-evaluates the closed-form 2x(6+3+1) blocks from 8-byte
 //     observations (ba_math.cuh) -- HBM traffic per LM iteration is the observation list + the point/camera state.
 //   * ba_point_kernel   (K3a, point-major, one sub-warp group per 3D point): U_p = sum Jp^T Jp + D_p^2, its Cholesky

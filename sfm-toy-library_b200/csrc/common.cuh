@@ -67,7 +67,7 @@ struct BAWorkspace {
 };
 
 // Descriptor images kept resident between per-call matchFeatures invocations (match.cu): one arena of packed rows, one of
-// expanded tcgen05 operand blocks, bump-allocated, flushed whole when full.
+// expanded tensor-core operand blocks, bump-allocated, flushed whole when full.
 struct MatchCacheEntry { const void* host; int rows; int desc_bytes; uint64_t hash; int row0; int blk0; };
 struct MatchCache {
     DevBuf desc, exp;

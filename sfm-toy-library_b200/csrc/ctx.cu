@@ -28,8 +28,8 @@ int sfmb200_create(int device, sfmb200_ctx** out) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
     if (e != cudaSuccess) return sfmb200_fail(nullptr, SFMB200_ERR_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 10)
-        return sfmb200_fail(nullptr, SFMB200_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_100a (B200) only",
+    if (prop.major != 9 || prop.minor != 0)
+        return sfmb200_fail(nullptr, SFMB200_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_90a (H100) only",
                             device, prop.major, prop.minor);
     sfmb200_ctx* c = new sfmb200_ctx();
     c->device = device; c->sm_count = prop.multiProcessorCount;

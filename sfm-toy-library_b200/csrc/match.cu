@@ -143,7 +143,7 @@ merge_flag_scan_kernel(const int4* __restrict__ partial, int splits, int64_t row
                 if (p.w >= 0) top2_insert(b, p.z, p.w);
             }
             i0 = b.i0; i1 = b.i1; fd0 = (float)b.d0; fd1 = (float)b.d1;          // DMatch.distance is float
-            // is_l2 == 2: exact integer SQUARED L2 distances (tcgen05 u8 GEMM); cv::batchDistance returns sqrt of the float sum
+            // is_l2 == 2: exact integer SQUARED L2 distances (wgmma u8 GEMM); cv::batchDistance returns sqrt of the float sum
             if (is_l2 == 2) { fd0 = sqrtf(fd0); fd1 = sqrtf(fd1); }
         } else {
             float d0 = 3.4e38f, d1 = 3.4e38f;
@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_sums_kernel(int32_t* __rest
         if (threadIdx.x == 0) carry_s = carry + total;
         __syncthreads();
     }
-    // a tcgen05 pipeline error (bounded mbarrier wait expired) poisons the total: device-resident callers see -1
+    // a tensor-core pipeline error (bounded mbarrier wait expired) poisons the total: device-resident callers see -1
     if (threadIdx.x == 0) *grand_total = (error_flag && *error_flag) ? -1 : carry_s;
 }
 
@@ -216,7 +216,7 @@ struct sfmb200_descset {
     uint32_t* d_desc = nullptr;
     std::vector<int32_t> img_off;
     int n_img = 0, words = 0, max_rows = 0;
-    // tcgen05 path (32-byte Hamming descriptors, u8-valued L2 descriptors): operands expanded once, blocks of 256 rows
+    // tensor-core path (32-byte Hamming descriptors, u8-valued L2 descriptors): operands expanded once, blocks of 256 rows
     uint8_t* d_exp = nullptr;
     std::vector<int32_t> img_blk;      // first block of each image
     int kind = 0;                      // 0 = Hamming, 1 = L2 (exact u8 GEMM)
@@ -500,7 +500,7 @@ static int match_pairs_host_out(sfmb200_ctx* ctx, const uint32_t* d_desc, const 
     int h_tc_err = 0;
     if (d_tc_err) SFM_CUDA(ctx, cudaMemcpyAsync(&h_tc_err, d_tc_err, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (h_tc_err) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "tcgen05 matcher: an MMA completion barrier timed out");
+    if (h_tc_err) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "tensor-core matcher: a pipeline barrier timed out");
     const int64_t total = *h_total;
     std::vector<int32_t> starts_copy(h_start, h_start + n_pairs);          // the staging buffer may move when it grows
     SFM_CUDA(ctx, ctx->pinned.reserve(head + 12 * (size_t)total));

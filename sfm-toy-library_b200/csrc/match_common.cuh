@@ -1,4 +1,4 @@
-// match_common.cuh -- types shared by the two Hamming knn2 kernels (match.cu: XOR/POPC, match_tc.cu: tcgen05) and their epilogue.
+// match_common.cuh -- types shared by the two Hamming knn2 kernels (match.cu: XOR/POPC, match_tc.cu: wgmma) and their epilogue.
 #pragma once
 #include "common.cuh"
 #include <climits>
@@ -7,7 +7,7 @@ struct PairDesc {          // one (left,right) image pair
     int q_row, nq;         // rows of the left image inside the descriptor array
     int t_row, nt;         // rows of the right image
     int64_t out_row;       // first row of this pair in the flattened [sum nq] arrays
-    int q_blk, t_blk;      // first 256-row block of the left / right image in the expanded operand store (tcgen05 path)
+    int q_blk, t_blk;      // first 256-row block of the left / right image in the expanded operand store (tensor-core path)
 };
 
 struct Top2 { int d0, i0, d1, i1; };
@@ -18,7 +18,7 @@ __device__ __forceinline__ void top2_insert(Top2& b, int d, int j) {
     else if (d < b.d1) { b.d1 = d; b.i1 = j; }
 }
 
-// tcgen05 path (match_tc.cu): Hamming on 32-byte descriptors, L2 on u8-valued descriptors of dimension <= 128
+// tensor-core path (match_tc.cu): Hamming on 32-byte descriptors, L2 on u8-valued descriptors of dimension <= 128
 int match_tc_splits(int sm_count, int n_pairs, int nq_max, int nt_max);
 size_t match_tc_block_bytes(bool l2);
 int match_tc_block_rows();

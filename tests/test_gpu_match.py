@@ -90,7 +90,7 @@ def test_config4_properties_full_size(ctx):
 
 @pytest.mark.parametrize("nq,nt", [(255, 257), (5000, 5000), (130, 9000), (4999, 513)])
 def test_popc_and_tensor_core_paths_are_bit_identical(ctx, oracle, monkeypatch, nq, nt):
-    """32-byte descriptors default to the tcgen05 integer-GEMM kernel (match_tc.cu); SFMB200_MATCH=popc forces the
+    """32-byte descriptors default to the wgmma integer-GEMM kernel (match_tc.cu); SFMB200_MATCH=popc forces the
     XOR/POPC kernel.  Both must reproduce the oracle exactly (indices, distances, tie-breaks)."""
     t = synth.make_descriptors(nt % 91, nt); q = synth.make_descriptors(nq % 83 + 200, nq, prev=t)
     t[5:9] = t[4]                                                            # duplicate train rows: tie-break inside one MMA tile
@@ -135,7 +135,7 @@ def test_cache_flush_when_arena_is_full(ctx, oracle):
 
 @pytest.mark.parametrize("nq,nt,dim", [(1, 2, 128), (300, 257, 128), (2000, 2100, 128), (5000, 5000, 128), (700, 650, 64), (129, 1000, 100)])
 def test_l2_exact_u8_gemm_vs_oracle(ctx, oracle, nq, nt, dim):
-    """SIFT-like (integer-valued) descriptors: the tcgen05 u8 x u8 -> s32 GEMM path (|a-b|^2 = |a|^2 + |b|^2 - 2<a,b>, exact)
+    """SIFT-like (integer-valued) descriptors: the wgmma u8 x u8 -> s32 GEMM path (|a-b|^2 = |a|^2 + |b|^2 - 2<a,b>, exact)
     gives the indices AND float distances of cv::BFMatcher(NORM_L2) (= the oracle's float loop, pinned to cv2 by the golden)."""
     t = synth.make_sift_like(nt % 50, nt, dim=dim); q = synth.make_sift_like(nq % 40 + 60, nq, dim=dim, prev=t)
     q[::7] = t[np.arange(len(q[::7])) % nt]                                   # exact duplicates: distance 0 and ties

@@ -1,7 +1,7 @@
 // tools/chol_microbench.cu -- K4 in isolation: the step-wise panel/update sequence against the dataflow kernel (with and
 // without lookahead) on an SPD matrix of the reduced-camera-system size, checked against a host factorisation, plus the
 // critical-path timeline of the dataflow kernel from its %globaltimer trace.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -o tools/_build/chol_microbench tools/chol_microbench.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -o tools/_build/chol_microbench tools/chol_microbench.cu
 // Usage: chol_microbench [cams=100] [reps=20]
 #include <algorithm>
 #include <cmath>

@@ -1,6 +1,6 @@
 // tools/fp64_peak.cu -- measured fp64 issue peaks of the device: DFMA (CUDA cores) and DMMA m8n8k4 (mma.sync f64).
 // These are the denominators for the "fp64" side of the BA roofline (MEASURED_PEAKS.json only carries HBM and bf16).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/_build/fp64_peak tools/fp64_peak.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/_build/fp64_peak tools/fp64_peak.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

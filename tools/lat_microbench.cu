@@ -1,6 +1,6 @@
 // tools/lat_microbench.cu -- dependent-issue latencies (cycles) of what the tile factorisation's pivot chain is made of:
 // DFMA, DMUL, the refined reciprocal square root, a shuffle, a shared-memory round trip, a 128-thread named barrier.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/_build/lat_microbench tools/lat_microbench.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/_build/lat_microbench tools/lat_microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -5,7 +5,7 @@
 //   mode 1: one 6x6 block per lane (28 lanes busy, 36 RED instructions, each touching 28 different blocks)
 //   mode 2: as mode 0 with plain stores instead of RED (upper bound of the store path)
 //   mode 3: as mode 0 but every warp hits the SAME block (same-address contention)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/_build/red_microbench tools/red_microbench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/_build/red_microbench tools/red_microbench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
