@@ -9,21 +9,20 @@
 //   * The Jacobian is never materialised.  Every pass re-evaluates the closed-form 2x(6+3+1) blocks from 8-byte
 //     observations (ba_math.cuh) -- HBM traffic per LM iteration is the observation list + the point/camera state.
 //   * ba_point_kernel   (K3a, point-major, one sub-warp group per 3D point): U_p = sum Jp^T Jp + D_p^2, its Cholesky
-//     inverse M_p, g_p, and per observation Z_o = Jc^T Jp M^T (Zbuf).
-//   * ba_row_kernel     (K3b, camera-major, ba_row.cuh): a CTA walks a slice of the STABLE camera-sorted observation list and
-//     keeps the block row S[ci, ci+1..] of the camera it is in in shared memory: the off-diagonal blocks  S[ci,cj] -= sum
-//     Z_i Z_j^T  come from the records that FOLLOW Z_i in the point-major Z buffer (one mma.sync.m8n8k4.f64 per update, no index
-//     lists, no atomics), the diagonal block, the camera-focal column the shared focal creates (SURVEY.md section 0-2), rhs,
-//     gradient and J^T J diagonal from two 8x8 fp64 tensor-core products per warp.  ba_combine_kernel sums the per-(slice,
-//     camera) partial records in a fixed order: no floating-point atomics, bitwise reproducible.
-//     ("red" mode, SFMB200_BA_SCHUR=red or more cameras than a shared-memory row holds, keeps the per-point
+//     inverse M_p, g_p, and per observation Z_o = Jc^T Jp M^T (Zbuf, 144 bytes per observation).
+//   * ba_pair_kernel    (K3c, ba_row.cuh): the off-diagonal blocks  S[ci,cj] -= sum Z_i Z_j^T  from per-(camera pair, point
+//     segment) entry lists sorted by point, one mma.sync.m8n8k4.f64 per entry, one partial block per (pair, segment, split).
+//   * ba_camera_kernel<DET> (camera-major slices of the stable camera-sorted list): diagonal blocks, camera-focal column, rhs,
+//     gradient and J^T J diagonal, one partial record per (slice, camera).  ba_combine_kernel sums the partial blocks and
+//     records in a fixed order: no floating-point atomics, bitwise reproducible.
+//     ("red" mode, SFMB200_BA_SCHUR=red or more cameras than the partial buffers allow, keeps the per-point
 //     red.global.add.f64 formulation with the register-accumulating ba_camera_kernel.)
 //   * reduced system summed over ranks: peer-memory kernel (loads the peers' buffers over NVLink into a local summed copy)
 //     or one NCCL all-reduce (S, rhs, gradient, diag, cost in one buffer).
 //   * ba_assemble + chol.cuh (streaming dataflow tile Cholesky, rhs carried as an extra row so the forward substitution is
 //     free, staged back substitution with inverse diagonal tiles): K4.
-//   * ba_backsub_z_kernel (point-major): delta_p from the stored Z blocks, candidate point, model cost change and candidate
-//     cost fused, no Jacobian re-evaluation.
+//   * ba_backsub_eval_kernel (point-major, default): delta_p from Jacobians re-evaluated at x, candidate point, model cost
+//     change and candidate cost fused; ba_backsub_z_kernel (SFMB200_BA_BACKSUB=stored) reads the stored Z blocks instead.
 //   LM control runs on the DEVICE (LMState, ba_lm_control_kernel); the host enqueues chunks of iterations and reads the
 //   state back once per chunk.
 #include "common.cuh"
@@ -378,7 +377,7 @@ __global__ void __launch_bounds__(PT_THREADS, 3) ba_point_kernel(BAView v, doubl
                 W[a * 3] = w0 * M[0]; W[a * 3 + 1] = w0 * M[1] + w1 * M[2]; W[a * 3 + 2] = w0 * M[3] + w1 * M[4] + w2 * M[5];
             }
         }
-        if (GATHER) continue;           // off-diagonal blocks are accumulated by ba_row_kernel from Zbuf
+        if (GATHER) continue;           // off-diagonal blocks are accumulated by ba_pair_kernel from Zbuf
         __syncwarp();
         // pair sweep: the whole warp handles the points of its GW groups one after the other
 #pragma unroll 1
@@ -427,7 +426,7 @@ __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, do
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// K3b ("red" mode only; the default is ba_row_kernel, ba_row.cuh): camera-major pass over the camera-sorted observation list.  Every CTA takes an equal, contiguous slice of the list
+// K3b (DET = false in "red" mode; DET = true in gather mode, summed by ba_combine_kernel): camera-major pass over the camera-sorted observation list.  Every CTA takes an equal, contiguous slice of the list
 // (grid = number of co-resident CTAs, one balanced wave; a per-camera grid left a third of the run to a ragged last wave)
 // and walks the cameras its slice touches.  Per camera: diagonal block, camera-focal column, rhs, gradient and J^T J
 // diagonal, all in registers; one reduction per (CTA, camera).
@@ -571,7 +570,7 @@ __global__ void ba_assemble_kernel(const double* __restrict__ Sblk, const double
 
 // cameras + focal: candidate = x - y*scale ; derived table of the candidate ; norms.  Single CTA.
 // locals[0] = |delta_cf|^2, [1] = |x_cf|^2, [2] = |cand_cf|^2, [3] = max |g_cf| (unscaled), [4] = camera part of -model cost change; post[7] = max |g_pts| (max-reduced over ranks)
-__global__ void __launch_bounds__(256) ba_cam_update_kernel(BAView v, double inv_radius, int model_from_step, const double* x_cf, const double* __restrict__ y_cf,
+__global__ void __launch_bounds__(256) ba_cam_update_kernel(BAView v, double inv_radius, const double* x_cf, const double* __restrict__ y_cf,
                                                             const double* __restrict__ scale_cf, const double* __restrict__ gcf, int nc,
                                                             double* cand_cf, CamDerived* camd_c, double* __restrict__ locals,
                                                             double* __restrict__ post, const unsigned long long* __restrict__ gmax_pt_bits,
@@ -600,7 +599,7 @@ __global__ void __launch_bounds__(256) ba_cam_update_kernel(BAView v, double inv
     if (threadIdx.x == 0) {
         double s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0;
         for (int w = 0; w < 8; ++w) { s0 += red[w][0]; s1 += red[w][1]; s2 += red[w][2]; s3 = fmax(s3, red[w][3]); s4 += red[w][4]; }
-        locals[0] = s0; locals[1] = s1; locals[2] = s2; locals[3] = s3; locals[4] = model_from_step ? s4 : 0.0;
+        locals[0] = s0; locals[1] = s1; locals[2] = s2; locals[3] = s3; locals[4] = s4;
         // rank-local flags -> buffers that are reduced over ranks (sum / max) so that every rank takes the same decision
         post[7] = __longlong_as_double((long long)*gmax_pt_bits);      // max-reduced over ranks
         post[4] = (double)fail[0]; post[5] = (double)fail[1];
@@ -812,53 +811,92 @@ __global__ void __launch_bounds__(PT_THREADS) ba_backsub_z_kernel(BAView v, doub
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Back substitution for the points + step evaluation, fused (point-major, same grouping as K3a):
-//   y_p = M^T (zg - M sum_o Jp^T (Jc y_c + Jf y_f)) ;  candidate X' = X - y_p*scale
-//   model cost change accumulates  m.(r + m/2)  with m = J*step ;  candidate cost from the residual at the candidate.
-// post[0] = sum r'^2, post[1] = sum m.(r+m/2), post[2] = |delta_pts|^2, post[3] = |cand_pts|^2
+// Back substitution for the points + step evaluation from re-evaluated Jacobians (default; no Z blocks are read):
+//     y_p = M^T (zg - M t),   t = sum_o Jp^T (Jc y_c + Jf y_f)        [ M t = sum_o Z_o^T y_c + zf y_f ]
+// One closed-form Jacobian at x per observation (~300 flop) instead of a 144-byte Z record, then the residual at the candidate.
+// The model cost change is the same 1/2 y.(g + D^2 y) as in ba_backsub_z_kernel (point part here, camera/focal part in
+// ba_cam_update_kernel), so the Jacobian is not needed a second time.
+// Per-camera operands (CamDerived at x, candidate rotation + translation, scaled y_c) sit in shared memory when they fit
+// (CAMTAB); the next iteration's lines are prefetched into L2 and its CSR offsets loaded one iteration ahead, as in
+// ba_backsub_z_kernel.
+// post[0] = sum r'^2, post[1] = -(point part of the model cost change), post[2] = |delta_pts|^2, post[3] = |cand_pts|^2
 // ---------------------------------------------------------------------------------------------------------------
-template <int G>
-__global__ void __launch_bounds__(PT_THREADS) ba_backsub_eval_kernel(BAView v, const double* __restrict__ y_cf, const double* cand_cf,
-                                                                     const CamDerived* camd_c, double* pts_c,
-                                                                     double* __restrict__ post) {
+struct BacksubCam {
+    CamDerived d;                  // at x
+    double Rc[9], tc[3];           // candidate rotation and translation
+    double ys[6];                  // scale_cf * y_c
+};
+template <int G, bool CAMTAB>
+__global__ void __launch_bounds__(PT_THREADS) ba_backsub_eval_kernel(BAView v, double inv_radius, const double* __restrict__ y_cf, const double* cand_cf,
+                                                                     const CamDerived* camd_c, double* pts_c, double* __restrict__ post) {
+    extern __shared__ __align__(16) unsigned char bs_smem[];
+    BacksubCam* camtab = reinterpret_cast<BacksubCam*>(bs_smem);     // [nc] (CAMTAB)
     const LMX x = lm_x(v);
     if (!x.run) return;
-    if (v.st) { const int nxt = v.st->cur ^ 1; cand_cf = v.cf2[nxt]; camd_c = v.camd2[nxt]; pts_c = v.pts2[nxt]; }
+    if (v.st) { const int nxt = v.st->cur ^ 1; cand_cf = v.cf2[nxt]; camd_c = v.camd2[nxt]; pts_c = v.pts2[nxt]; inv_radius = 1.0 / v.st->radius; }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, gl = lane % G;
     const unsigned gmask = G == 32 ? 0xffffffffu : (((1u << G) - 1u) << ((lane / G) * G));
     constexpr int GB = PT_THREADS / G;
-    const double f = *x.focal, sf = v.scale_cf[6 * v.nc], yf = y_cf[6 * v.nc], fc = cand_cf[6 * v.nc];
+    const double f = *x.focal, yfs = v.scale_cf[6 * v.nc] * y_cf[6 * v.nc], fc = cand_cf[6 * v.nc];
+    if (CAMTAB) {
+        constexpr int CD = sizeof(CamDerived) / 8, CT = sizeof(BacksubCam) / 8;
+        double* tab = reinterpret_cast<double*>(bs_smem);
+        for (int i = threadIdx.x; i < v.nc * CT; i += PT_THREADS) {
+            const int c = i / CT, q = i - CT * c;
+            tab[i] = q < CD ? reinterpret_cast<const double*>(x.camd + c)[q]
+                   : q < CD + 12 ? reinterpret_cast<const double*>(camd_c + c)[q - CD]
+                   : v.scale_cf[6 * c + q - CD - 12] * y_cf[6 * c + q - CD - 12];
+        }
+        __syncthreads();
+    }
     double acc_cc = 0, acc_m = 0, acc_dn = 0, acc_cn = 0;
-    for (int p = blockIdx.x * GB + threadIdx.x / G; p < v.np; p += gridDim.x * GB) {
-        const int o0 = v.pt_off[p], k = v.pt_off[p + 1] - o0;
-        const double X[3] = {x.pts[3 * p], x.pts[3 * p + 1], x.pts[3 * p + 2]};
-        const double sp[3] = {v.scale_pt[3 * p], v.scale_pt[3 * p + 1], v.scale_pt[3 * p + 2]};
-        const double* pb = v.ptblk + (size_t)p * PTB;
-        const double M[6] = {pb[0], pb[1], pb[2], pb[3], pb[4], pb[5]};
-        const double zg[3] = {pb[6], pb[7], pb[8]};
-        // pass 1: t = sum_o Jp^T (Jc y_c + Jf y_f).  For the lane's first observation the pieces pass 2 needs
-        // (m' = Jc y_c + Jf y_f, Jp, r) stay in registers, so the Jacobian is evaluated once per observation.
+    const int np_round = (v.np + GB - 1) / GB * GB;
+    int o0_next = 0, k_next = 0;
+    { const int pn = blockIdx.x * GB + threadIdx.x / G; if (pn < v.np) { o0_next = v.pt_off[pn]; k_next = v.pt_off[pn + 1] - o0_next; } }
+    for (int p0 = blockIdx.x * GB; p0 < np_round; p0 += gridDim.x * GB) {
+        const int p = p0 + threadIdx.x / G;
+        const bool active = p < v.np;
+        const int o0 = o0_next, k = k_next;
+        {
+            const int pn = p + gridDim.x * GB;
+            o0_next = 0; k_next = 0;
+            if (pn < v.np) {
+                o0_next = v.pt_off[pn]; k_next = v.pt_off[pn + 1] - o0_next;
+                if (gl == 0) {
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(v.obs_cam + o0_next)); asm volatile("prefetch.global.L2 [%0];" :: "l"(v.obs_xy + o0_next));
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(x.pts + 3 * (size_t)pn)); asm volatile("prefetch.global.L2 [%0];" :: "l"(v.scale_pt + 3 * (size_t)pn));
+                    const char* pbn = reinterpret_cast<const char*>(v.ptblk + (size_t)pn * PTB);
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(pbn)); asm volatile("prefetch.global.L2 [%0];" :: "l"(pbn + 128));
+                }
+            }
+        }
+        double X[3] = {0, 0, 0};
+        if (active) { X[0] = x.pts[3 * p]; X[1] = x.pts[3 * p + 1]; X[2] = x.pts[3 * p + 2]; }
+        // pass 1: t = sum_o Jp^T (Jc y_c + Jf y_f), Jacobians unscaled; the scaling is folded into ys, yfs and sp
         double t[3] = {0, 0, 0};
-        double k_m0 = 0, k_m1 = 0, k_r0 = 0, k_r1 = 0, k_Jp[6] = {0, 0, 0, 0, 0, 0};
         for (int j = gl; j < k; j += G) {
             const int o = o0 + j, c = v.obs_cam[o];
-            ObsJ J;
-            eval_scaled(x.camd[c], X, f, v.obs_xy[o], v.scale_cf + 6 * c, sp, sf, J);
-            double m0 = J.Jf[0] * yf, m1 = J.Jf[1] * yf;
+            const float2 xy = v.obs_xy[o];
+            double r[2], Jc[12], Jp[6], Jf[2];
+            obs_eval(CAMTAB ? camtab[c].d : x.camd[c], X, f, (double)xy.x, (double)xy.y, r, Jc, Jp, Jf);
+            double m0 = Jf[0] * yfs, m1 = Jf[1] * yfs;
 #pragma unroll
-            for (int a = 0; a < 6; ++a) { const double yc = y_cf[6 * c + a]; m0 += J.Jc[a] * yc; m1 += J.Jc[6 + a] * yc; }
-#pragma unroll
-            for (int a = 0; a < 3; ++a) t[a] += J.Jp[a] * m0 + J.Jp[3 + a] * m1;
-            if (j == gl) {
-                k_m0 = m0; k_m1 = m1; k_r0 = J.r[0]; k_r1 = J.r[1];
-#pragma unroll
-                for (int a = 0; a < 6; ++a) k_Jp[a] = J.Jp[a];
+            for (int a = 0; a < 6; ++a) {
+                const double ys = CAMTAB ? camtab[c].ys[a] : v.scale_cf[6 * c + a] * y_cf[6 * c + a];
+                m0 += Jc[a] * ys; m1 += Jc[6 + a] * ys;
             }
+#pragma unroll
+            for (int a = 0; a < 3; ++a) t[a] += Jp[a] * m0 + Jp[3 + a] * m1;
         }
 #pragma unroll
         for (int a = 0; a < 3; ++a) t[a] = group_sum<G>(t[a], gmask);
+        if (!active) continue;
+        const double sp[3] = {v.scale_pt[3 * p], v.scale_pt[3 * p + 1], v.scale_pt[3 * p + 2]};
+        t[0] *= sp[0]; t[1] *= sp[1]; t[2] *= sp[2];
+        const double* pb = v.ptblk + (size_t)p * PTB;
+        const double M[6] = {pb[0], pb[1], pb[2], pb[3], pb[4], pb[5]};
         // u = zg - M t ; y_p = M^T u
-        const double u0 = zg[0] - M[0] * t[0], u1 = zg[1] - (M[1] * t[0] + M[2] * t[1]), u2 = zg[2] - (M[3] * t[0] + M[4] * t[1] + M[5] * t[2]);
+        const double u0 = pb[6] - M[0] * t[0], u1 = pb[7] - (M[1] * t[0] + M[2] * t[1]), u2 = pb[8] - (M[3] * t[0] + M[4] * t[1] + M[5] * t[2]);
         const double yp[3] = {M[0] * u0 + M[1] * u1 + M[3] * u2, M[2] * u1 + M[4] * u2, M[5] * u2};
         const double Xc[3] = {X[0] - yp[0] * sp[0], X[1] - yp[1] * sp[1], X[2] - yp[2] * sp[2]};
         if (gl == 0) {
@@ -866,29 +904,22 @@ __global__ void __launch_bounds__(PT_THREADS) ba_backsub_eval_kernel(BAView v, c
             const double d0 = X[0] - Xc[0], d1 = X[1] - Xc[1], d2 = X[2] - Xc[2];
             acc_dn += d0 * d0 + d1 * d1 + d2 * d2;
             acc_cn += Xc[0] * Xc[0] + Xc[1] * Xc[1] + Xc[2] * Xc[2];
+#pragma unroll
+            for (int a = 0; a < 3; ++a) acc_m -= 0.5 * yp[a] * (pb[12 + a] + clampd(pb[15 + a], v.min_diag, v.max_diag) * inv_radius * yp[a]);
         }
-        // pass 2: model residual m = -J y and candidate residual
+        // pass 2: residual at the candidate
         for (int j = gl; j < k; j += G) {
             const int o = o0 + j, c = v.obs_cam[o];
             const float2 xy = v.obs_xy[o];
-            double m0, m1, r0, r1;
-            if (j == gl) {
-                m0 = k_m0; m1 = k_m1; r0 = k_r0; r1 = k_r1;
-#pragma unroll
-                for (int a = 0; a < 3; ++a) { m0 += k_Jp[a] * yp[a]; m1 += k_Jp[3 + a] * yp[a]; }
-            } else {
-                ObsJ J;
-                eval_scaled(x.camd[c], X, f, xy, v.scale_cf + 6 * c, sp, sf, J);
-                m0 = J.Jf[0] * yf; m1 = J.Jf[1] * yf; r0 = J.r[0]; r1 = J.r[1];
-#pragma unroll
-                for (int a = 0; a < 6; ++a) { const double yc = y_cf[6 * c + a]; m0 += J.Jc[a] * yc; m1 += J.Jc[6 + a] * yc; }
-#pragma unroll
-                for (int a = 0; a < 3; ++a) { m0 += J.Jp[a] * yp[a]; m1 += J.Jp[3 + a] * yp[a]; }
-            }
-            m0 = -m0; m1 = -m1;
-            acc_m += m0 * (r0 + 0.5 * m0) + m1 * (r1 + 0.5 * m1);
             double rc[2];
-            obs_residual(camd_c[c], Xc, fc, (double)xy.x, (double)xy.y, rc);
+            if (CAMTAB) {
+                const double* Rc = camtab[c].Rc; const double* tc = camtab[c].tc;       // same arithmetic as obs_residual
+                const double q0 = Rc[0] * Xc[0] + Rc[1] * Xc[1] + Rc[2] * Xc[2] + tc[0];
+                const double q1 = Rc[3] * Xc[0] + Rc[4] * Xc[1] + Rc[5] * Xc[2] + tc[1];
+                const double q2 = Rc[6] * Xc[0] + Rc[7] * Xc[1] + Rc[8] * Xc[2] + tc[2];
+                const double iz = 1.0 / q2;
+                rc[0] = fc * (q0 * iz) - (double)xy.x; rc[1] = fc * (q1 * iz) - (double)xy.y;
+            } else obs_residual(camd_c[c], Xc, fc, (double)xy.x, (double)xy.y, rc);
             acc_cc += rc[0] * rc[0] + rc[1] * rc[1];
         }
     }
@@ -896,10 +927,10 @@ __global__ void __launch_bounds__(PT_THREADS) ba_backsub_eval_kernel(BAView v, c
     const double c0 = warp_sum(acc_cc), c1 = warp_sum(acc_m), c2 = warp_sum(acc_dn), c3 = warp_sum(acc_cn);
     if (lane == 0) { sred[warp][0] = c0; sred[warp][1] = c1; sred[warp][2] = c2; sred[warp][3] = c3; }
     __syncthreads();
-    double t[4] = {0, 0, 0, 0};
-    if (threadIdx.x == 0) for (int w = 0; w < PT_THREADS / 32; ++w) { t[0] += sred[w][0]; t[1] += sred[w][1]; t[2] += sred[w][2]; t[3] += sred[w][3]; }
+    double tt[4] = {0, 0, 0, 0};
+    if (threadIdx.x == 0) for (int w = 0; w < PT_THREADS / 32; ++w) { tt[0] += sred[w][0]; tt[1] += sred[w][1]; tt[2] += sred[w][2]; tt[3] += sred[w][3]; }
     double tot[4];
-    if (last_block_sum4(v.part4, v.counters + 1, t, tot) && threadIdx.x == 0) { post[0] = tot[0]; post[1] = tot[1]; post[2] = tot[2]; post[3] = tot[3]; }
+    if (last_block_sum4(v.part4, v.counters + 1, tt, tot) && threadIdx.x == 0) { post[0] = tot[0]; post[1] = tot[1]; post[2] = tot[2]; post[3] = tot[3]; }
 }
 
 // camera-major copy of the observation list: counting sort by camera (structure is fixed across LM iterations).
@@ -1030,13 +1061,13 @@ struct sfmb200_ba_problem {
     unsigned* solve_counter = nullptr;   // device-side number of the current dense solve (incremented by ba_assemble_kernel)
     double* h_scal = nullptr;         // pinned read-back: sums[8] post[8] locals[8] gmax fail
     bool have_scale = false;
-    bool backsub_from_z = false;      // back-substitution + model cost from the stored Z blocks (gather mode) instead of re-evaluated Jacobians
+    bool backsub_from_z = false;      // back-substitution from the stored Z blocks (gather mode, Zbuf within one L2-sized segment) instead of re-evaluated Jacobians
     bool camd_valid[2] = {false, false};   // camd[i] matches cf[i] (written by cam_derive or, for the candidate, by ba_cam_update_kernel)
     EvSet evs[LM_CHUNK_MAX];              // profile mode: one set of events per iteration of a chunk (created on first use)
     bool have_events = false;
     LMState* d_state = nullptr; LMState* h_state = nullptr;    // device-resident LM control state + pinned read-back
     // row mode (default): Z per observation (point-major), stable camera-major list with follower counts, partial records
-    bool gather = true;               // true = row mode (ba_row_kernel), false = "red" mode
+    bool gather = true;               // true = gather mode (ba_pair_kernel + partial records), false = "red" mode
     double* Zbuf = nullptr;
     int32_t* obs_pt = nullptr; int32_t* cm_obs = nullptr; uint8_t* cm_np = nullptr;
     double* diag_part = nullptr; int diag_grid = 0, diag_per_cta = 0;
@@ -1079,6 +1110,14 @@ static RowArgs make_row_args(const sfmb200_ba_problem* P) {
     ra.pair_off = P->pair_off; ra.pair_part = P->pair_part; ra.nseg = P->pair_nseg; ra.splits = P->pair_splits;
     ra.pair_blk = P->pair_blk; ra.n_nonempty = P->n_pairs_nonempty;
     return ra;
+}
+
+// Point segments of the pair accumulation: Zbuf (144 bytes per observation) in slices of a quarter of the L2 cache, so that the
+// slice all resident warps of ba_pair_kernel read stays L2-resident next to the streamed entry lists (H100: 50 MB L2 in two
+// partitions -> 12.5 MB slices).
+static int pair_segments(const sfmb200_ctx* ctx, int nobs) {
+    const long long seg = std::max(ctx->l2_bytes, 8 << 20) / 4;
+    return (int)std::max<long long>(1, std::min<long long>(64, (144LL * nobs + seg - 1) / seg));
 }
 
 static size_t point_smem_bytes(int G, int maxk) {
@@ -1134,9 +1173,15 @@ template <int G> static int launch_backsub(sfmb200_ba_problem* P, const BAView& 
             const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
             ba_backsub_z_kernel<G, false><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
         }
-    } else {
-        const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
-        ba_backsub_eval_kernel<G><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
+    } else {                            // default: Jacobians re-evaluated at x (no Z blocks)
+        const size_t tab = sizeof(BacksubCam) * (size_t)P->nc;
+        if (tab <= 40 * 1024) {
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB), 16);
+            ba_backsub_eval_kernel<G, true><<<blocks, PT_THREADS, tab, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
+        } else {
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
+            ba_backsub_eval_kernel<G, false><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
+        }
     }
     SFM_LAUNCH_CHECK(ctx);
     return SFMB200_OK;
@@ -1470,12 +1515,12 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         }
     }
     CRT(cudaMemsetAsync(P->counters, 0, 64, st));
-    {   // mode: "row" (default: ba_row_kernel, deterministic) needs the block row of a camera (288 bytes per camera) in shared
+    {   // mode: gather (default: ba_pair_kernel + ba_combine_kernel, deterministic) needs the pair-list fill's per-warp camera counters in shared
         // memory and the stable sort's per-warp counters; "red" (SFMB200_BA_SCHUR=red, or too many cameras) uses atomics
         const char* mode = getenv("SFMB200_BA_SCHUR");
         // partial blocks of the pair kernel: one 288-byte block per (camera pair, point segment[, split]); with thousands of cameras
         // that buffer (and the per-key offset tables) outgrow their use -- such problems take the atomics path
-        const size_t nseg_est = (size_t)std::max<long long>(1, std::min<long long>(64, (144LL * nobs + (24LL << 20) - 1) / (24LL << 20)));
+        const size_t nseg_est = (size_t)pair_segments(ctx, nobs);
         const bool partials_fit = nblk * nseg_est * 288 <= ((size_t)256 << 20);
         P->gather = !(mode && strcmp(mode, "red") == 0) && (size_t)(2 * PFILL_WARPS + 1) * nc * 4 <= 160 * 1024 && pair_entries < (1LL << 31) - 1024 && partials_fit;
     }
@@ -1502,10 +1547,10 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
             P->diag_per_cta = ceil_div(nobs, P->diag_grid);
             P->diag_grid = ceil_div(nobs, P->diag_per_cta);
         }
-        // off-diagonal blocks: per-(camera pair, point segment) entry lists, ~24 MB of Zbuf per segment so that one segment stays
-        // L2-resident while it is read ~7 times; one partial block per (pair, segment, split) warp
+        // off-diagonal blocks: per-(camera pair, point segment) entry lists, one segment of Zbuf small enough to stay L2-resident
+        // while it is read ~7 times (pair_segments); one partial block per (pair, segment, split) warp
         const long long E = pair_entries;           // observation pairs of a point, counted by the validation sweep
-        const int nseg = (int)std::max<long long>(1, std::min<long long>(64, (144LL * nobs + (24LL << 20) - 1) / (24LL << 20)));
+        const int nseg = pair_segments(ctx, nobs);
         const size_t nkeys = nblk * (size_t)nseg;
         // splits are fixed before the lists exist (they size the partial buffer): assume every pair is non-empty
         P->pair_nseg = nseg;
@@ -1562,7 +1607,11 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
             P->Zbuf = (double*)P->gmem.p;
         }
         const char* bm = getenv("SFMB200_BA_BACKSUB");
-        P->backsub_from_z = P->gather && P->Zbuf && !(bm && strcmp(bm, "jacobian") == 0);
+        // Z blocks when all of Zbuf is one L2-sized pair segment (still L2-resident from the point pass, and the 64-register
+        // kernel fits a small problem in one wave); otherwise re-evaluated Jacobians save the 144-byte record per observation
+        // that would come from HBM.  SFMB200_BA_BACKSUB=stored / jacobian forces either.
+        const bool z_in_l2 = P->pair_nseg == 1;
+        P->backsub_from_z = P->gather && P->Zbuf && (bm ? strcmp(bm, "stored") == 0 : z_in_l2);
     }
 #undef CRT
     *out = P;
@@ -1767,7 +1816,7 @@ int sfmb200_ba_problem_run(sfmb200_ba_problem* P, const sfmb200_ba_options* opt_
         BAView v = make_view(P, &opt, true);
         {
             BAView vc = v; vc.dcf = summed(P, P->dcf);              // the rank-summed J^T J diagonal and gradient
-            ba_cam_update_kernel<<<1, 256, 0, ctx->stream>>>(vc, 0.0, P->backsub_from_z ? 1 : 0, nullptr, P->y_cf, P->scale_cf, summed(P, P->gcf), P->nc, nullptr, nullptr, P->locals,
+            ba_cam_update_kernel<<<1, 256, 0, ctx->stream>>>(vc, 0.0, nullptr, P->y_cf, P->scale_cf, summed(P, P->gcf), P->nc, nullptr, nullptr, P->locals,
                                                              P->post, P->gmax_pt_bits, P->fail);
         }
         SFM_LAUNCH_CHECK(ctx);

@@ -94,6 +94,7 @@ struct DescWorkspace {
 struct sfmb200_ctx {
     int device = 0;
     int sm_count = 0;
+    int l2_bytes = 0;           // L2 cache size (sizes the L2-resident working sets of the bundle adjustment)
     cudaStream_t stream = nullptr;
     std::string err;
     int64_t launches = 0;

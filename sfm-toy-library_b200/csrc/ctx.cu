@@ -32,7 +32,7 @@ int sfmb200_create(int device, sfmb200_ctx** out) {
         return sfmb200_fail(nullptr, SFMB200_ERR_UNSUPPORTED, "device %d is sm_%d%d; this build targets sm_90a (H100) only",
                             device, prop.major, prop.minor);
     sfmb200_ctx* c = new sfmb200_ctx();
-    c->device = device; c->sm_count = prop.multiProcessorCount;
+    c->device = device; c->sm_count = prop.multiProcessorCount; c->l2_bytes = prop.l2CacheSize;
     e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { delete c; return sfmb200_fail(nullptr, SFMB200_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
     *out = c;
