@@ -230,6 +230,57 @@ enum { SFMB200_MODEL_HOMOGRAPHY = 0, SFMB200_MODEL_ESSENTIAL = 1, SFMB200_MODEL_
 int sfmb200_ransac_score(sfmb200_ctx* ctx, int model, const float* a, const float* b, int n, const double* hyp, int nh, const double* aux9,
                          double threshold, int32_t* inlier_counts, int32_t* best_index, uint8_t* best_mask);
 
+/* ---- f-2: essential-matrix RANSAC and pose recovery, all on the device ----------------------------------------- */
+/*
+ * findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118):
+ *     E = findEssentialMat(left, right, focal, pp, RANSAC, 0.999, 1.0, mask);  recoverPose(E, left, right, R, t, focal, pp, mask);
+ * in one call.  Points are normalised x = ((double)px - cx) / focal with focal = K[0], (cx, cy) = (K[2], K[5]); the threshold
+ * becomes threshold_px / focal.  max_iters samples of 5 distinct correspondences are drawn from a counter-based generator
+ * (splitmix64 keyed by seed, sample and draw; a repeated index is redrawn), every sample is solved by the five-point
+ * solver (up to 10 E), every solution is scored with the Sampson error and inlier rule of sfmb200_ransac_score, and
+ * OpenCV's sequential loop (RANSACPointSetRegistrator::run) is replayed over the counts in sample order: a solution
+ * replaces the best one only if its count exceeds max(best count, 4), every improvement recomputes the sample budget with
+ * RANSACUpdateNumIters(confidence, outlier ratio, 5, budget), and the loop stops at the budget.  The result is what that
+ * loop returns on this sample sequence; cv:: draws its samples from its own RNG, so it agrees with cv:: only statistically.
+ * The pose is recoverPose's: E = U diag(s, s, 0) V^T, candidates [U W V^T | t], [U W^T V^T | t], [.. | -t], [.. | -t]
+ * with t = U[:, 2]; a point counts for a candidate when its DLT triangulation against [I|0] has Q2 Q3 > 0, depth < distance_thresh in
+ * the first camera, depth in (0, distance_thresh) in the second and its RANSAC inlier flag set; the first candidate whose count is
+ * >= all others wins.
+ *   K [9] float row-major; points / match_q / match_t as in sfmb200_triangulate (NULL, NULL = aligned).
+ *   E [9], R [9], t [3] double (unit-norm t); any may be NULL.  inlier_mask [m] = findEssentialMat's mask, pose_mask [m] =
+ *   recoverPose's (the pruning mask); either may be NULL.  opt NULL = defaults.  summary may be NULL.
+ *   m < 5 or no model: SFMB200_OK with summary.found = 0, E / R / t / masks zero.
+ *   m == 5: cv::findEssentialMat returns every solution of the one sample stacked (and the reference's recoverPose would then
+ *   fail on the 3n x 3 matrix); here the one sample goes through the same selection as every other call.
+ * Same seed, same inputs: bitwise-identical outputs.  One host synchronisation per call.
+ */
+typedef struct {
+    int max_iters;            /* 1000  cv::findEssentialMat default; >= 1 */
+    double confidence;        /* 0.999 (SfMStereoUtilities.cpp:97); in (0, 1) */
+    double threshold_px;      /* 1.0   (:97); > 0 */
+    double distance_thresh;   /* 50    cv::recoverPose default; > 0 */
+    uint64_t seed;            /* 0 */
+} sfmb200_essential_options;
+typedef struct {
+    int found;                /* 1: a model with more than 4 inliers */
+    int n_inliers;            /* inliers of E (findEssentialMat's mask) */
+    int n_good;               /* points that pass the cheirality test (recoverPose's return value) */
+    int iterations;           /* samples the sequential loop visited */
+    int n_samples;            /* samples drawn and solved */
+    int n_hypotheses;         /* solutions of all samples */
+} sfmb200_essential_summary;
+void sfmb200_essential_default_options(sfmb200_essential_options* opt);
+int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* pts_left, int n_left, const float* pts_right, int n_right,
+                                 const int32_t* match_q, const int32_t* match_t, int m, const sfmb200_essential_options* opt,
+                                 double* E, double* R, double* t, uint8_t* inlier_mask, uint8_t* pose_mask, sfmb200_essential_summary* summary);
+/* Test hooks.  sfmb200_five_point: the device five-point solver on ns given samples, x1 / x2 [ns][5][2] normalised coordinates ->
+ * E [ns][10][9] (unit Frobenius norm, real roots in ascending order), nsol [ns].
+ * sfmb200_essential_last_trace: the last sfmb200_find_camera_matrices call's samples [cap][5], solution counts nsol [cap] and
+ * per-solution inlier counts [cap * 10] in (sample, solution) order, for its first min(cap, n_samples) samples; any output may
+ * be NULL.  Returns that call's n_samples (0 before any call), or -1 on bad arguments. */
+int sfmb200_five_point(sfmb200_ctx* ctx, const double* x1, const double* x2, int ns, double* E, int32_t* nsol);
+int sfmb200_essential_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, int32_t* nsol, int32_t* counts);
+
 /* ---- f-3 ("next" row of SURVEY.md 8): ORB feature extraction, the step before matching ------------------------ */
 /*
  * SfM2DFeatureUtilities::extractFeatures (SfMToyLib/SfM2DFeatureUtilities.h:41-42, .cpp:46-51):

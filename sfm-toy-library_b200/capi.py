@@ -48,6 +48,19 @@ class BASummary(C.Structure):
         return d
 
 
+class EssentialOptions(C.Structure):
+    _fields_ = [("max_iters", C.c_int), ("confidence", C.c_double), ("threshold_px", C.c_double), ("distance_thresh", C.c_double),
+                ("seed", C.c_uint64)]
+
+
+class EssentialSummary(C.Structure):
+    _fields_ = [("found", C.c_int), ("n_inliers", C.c_int), ("n_good", C.c_int), ("iterations", C.c_int), ("n_samples", C.c_int),
+                ("n_hypotheses", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 def lib():
     """Load libsfmb200.so (built by build.py / __graft_entry__.build()).  No fallback."""
     global _lib
@@ -205,6 +218,44 @@ class Context:
                                                C.c_double(float(threshold)), _p(counts, C.c_int32), C.byref(best), _p(mask, C.c_uint8) if want_mask else None))
         return counts[:nh], int(best.value), mask[:n]
 
+    # ------------------------------------------------------------------ f-2 essential-matrix RANSAC + pose recovery
+    def find_camera_matrices(self, K, pts_left, pts_right, match_q=None, match_t=None, options=None, **kw):
+        """sfmb200_find_camera_matrices: findEssentialMat(RANSAC) + recoverPose on the device.  options: EssentialOptions or
+        keyword overrides of the defaults (max_iters, confidence, threshold_px, distance_thresh, seed).
+        Returns (E [3,3], R [3,3], t [3], inlier_mask [m], pose_mask [m], summary dict)."""
+        K = np.ascontiguousarray(K, np.float32).reshape(9)
+        L = np.ascontiguousarray(pts_left, np.float32).reshape(-1, 2); R = np.ascontiguousarray(pts_right, np.float32).reshape(-1, 2)
+        if match_q is not None:
+            match_q = np.ascontiguousarray(match_q, np.int32); match_t = np.ascontiguousarray(match_t, np.int32); m = match_q.shape[0]
+        else:
+            m = min(L.shape[0], R.shape[0])
+        o = options or essential_default_options(**kw)
+        E = np.zeros(9); Rm = np.zeros(9); t = np.zeros(3)
+        inl = np.zeros(max(m, 1), np.uint8); pm = np.zeros(max(m, 1), np.uint8); s = EssentialSummary()
+        self._check(lib().sfmb200_find_camera_matrices(self._h, _p(K, C.c_float), _p(L, C.c_float), L.shape[0], _p(R, C.c_float), R.shape[0],
+                                                       _p(match_q, C.c_int32), _p(match_t, C.c_int32), m, C.byref(o), _p(E, C.c_double),
+                                                       _p(Rm, C.c_double), _p(t, C.c_double), _p(inl, C.c_uint8), _p(pm, C.c_uint8), C.byref(s)))
+        return E.reshape(3, 3), Rm.reshape(3, 3), t, inl[:m], pm[:m], s.as_dict()
+
+    def five_point(self, x1, x2):
+        """sfmb200_five_point: x1, x2 [ns, 5, 2] normalised coordinates -> (E [ns, 10, 3, 3], nsol [ns])."""
+        x1 = np.ascontiguousarray(x1, np.float64).reshape(-1, 5, 2); x2 = np.ascontiguousarray(x2, np.float64).reshape(-1, 5, 2)
+        ns = x1.shape[0]
+        E = np.zeros((max(ns, 1), 10, 9)); n = np.zeros(max(ns, 1), np.int32)
+        self._check(lib().sfmb200_five_point(self._h, _p(x1, C.c_double), _p(x2, C.c_double), ns, _p(E, C.c_double), _p(n, C.c_int32)))
+        return E[:ns].reshape(ns, 10, 3, 3), n[:ns]
+
+    def essential_last_trace(self):
+        """sfmb200_essential_last_trace: (samples [S, 5], nsol [S], counts [sum nsol]) of the last find_camera_matrices call."""
+        f = lib().sfmb200_essential_last_trace
+        S = f(self._h, 0, None, None, None)
+        if S < 0:
+            raise SfmB200Error("sfmb200_essential_last_trace failed")
+        smp = np.zeros((max(S, 1), 5), np.int32); n = np.zeros(max(S, 1), np.int32); c = np.zeros(max(10 * S, 1), np.int32)
+        if f(self._h, S, _p(smp, C.c_int32), _p(n, C.c_int32), _p(c, C.c_int32)) != S:
+            raise SfmB200Error("sfmb200_essential_last_trace failed")
+        return smp[:S], n[:S], c[:int(n[:S].sum())]
+
     # ------------------------------------------------------------------ f-3 ORB extraction
     def orb_detect_and_compute(self, images, nfeatures=5000, capacity=None):
         """sfmb200_orb_detect_and_compute[_batch]: `ORB::create(nfeatures)->detectAndCompute` (SfM2DFeatureUtilities.cpp:39, 48).
@@ -310,6 +361,14 @@ def comm_unique_id():
 def ba_default_options(**kw):
     o = BAOptions()
     lib().sfmb200_ba_default_options(C.byref(o))
+    for k, v in kw.items():
+        setattr(o, k, v)
+    return o
+
+
+def essential_default_options(**kw):
+    o = EssentialOptions()
+    lib().sfmb200_essential_default_options(C.byref(o))
     for k, v in kw.items():
         setattr(o, k, v)
     return o

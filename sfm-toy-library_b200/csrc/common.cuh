@@ -120,6 +120,8 @@ struct sfmb200_ctx {
     std::vector<std::pair<std::array<uint8_t, 64>, void*>> ipc_cache;
     CommState* comm = nullptr;
     int rank = 0, nranks = 1;
+    DevBuf ess_trace;           // samples / solution counts / inlier counts of the last essential-matrix RANSAC (essential.cu)
+    int ess_trace_samples = 0;
 };
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);

@@ -40,6 +40,8 @@ public:
 
 class SfMStereoUtilities {
 public:
+    static bool findCameraMatricesFromMatch(const Intrinsics& intrinsics, const Matching& featureMatching, const Features& featuresLeft,
+                                            const Features& featuresRight, Matching& prunedMatches, cv::Matx34f& Pleft, cv::Matx34f& Pright);
     static bool triangulateViews(const Intrinsics& intrinsics, const ImagePair imagePair, const Matching& matches,
                                  const Features& featuresLeft, const Features& featuresRight, const cv::Matx34f& Pleft,
                                  const cv::Matx34f& Pright, PointCloud& pointCloud);

@@ -136,6 +136,43 @@ bool SfMStereoUtilities::triangulateViews(const Intrinsics& intrinsics, const Im
     return true;
 }
 
+#ifdef SFMB200_SHIM_ESSENTIAL      // define it to replace findCameraMatricesFromMatch (OpenCV's findEssentialMat + recoverPose) too
+// SfMStereoUtilities.cpp:74-118: essential-matrix RANSAC and pose recovery in one device call (sfmb200_find_camera_matrices).
+bool SfMStereoUtilities::findCameraMatricesFromMatch(const Intrinsics& intrinsics, const Matching& matches, const Features& featuresLeft,
+                                                     const Features& featuresRight, Matching& prunedMatches, cv::Matx34f& Pleft,
+                                                     cv::Matx34f& Pright) {
+    if (intrinsics.K.empty()) {
+        std::cerr << "Intrinsics matrix (K) must be initialized." << std::endl;
+        return false;
+    }
+    const int m = (int)matches.size();
+    float K[9];
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) K[3 * r + c] = intrinsics.K.at<float>(r, c);
+    std::vector<int32_t> mq(m), mt(m);
+    for (int i = 0; i < m; ++i) { mq[i] = matches[i].queryIdx; mt[i] = matches[i].trainIdx; }
+    double R[9], t[3];
+    std::vector<uint8_t> pose_mask(m);
+    sfmb200_essential_summary summary;
+    check(sfmb200_find_camera_matrices(context(), K, reinterpret_cast<const float*>(featuresLeft.points.data()), (int)featuresLeft.points.size(),
+                                       reinterpret_cast<const float*>(featuresRight.points.data()), (int)featuresRight.points.size(),
+                                       mq.data(), mt.data(), m, nullptr, nullptr, R, t, nullptr, pose_mask.data(), &summary),
+          "sfmb200_find_camera_matrices");
+    if (!summary.found) {
+        std::cerr << "findCameraMatricesFromMatch: no essential matrix with more than 4 inliers among " << m << " matches" << std::endl;
+        return false;
+    }
+    Pleft = cv::Matx34f::eye();
+    for (int r = 0; r < 3; ++r) {                                                      // :105-107
+        for (int c = 0; c < 3; ++c) Pright(r, c) = (float)R[3 * r + c];
+        Pright(r, 3) = (float)t[r];
+    }
+    prunedMatches.clear();
+    for (int i = 0; i < m; ++i)
+        if (pose_mask[i]) prunedMatches.push_back(matches[i]);
+    return true;
+}
+#endif  // SFMB200_SHIM_ESSENTIAL
+
 void SfMBundleAdjustmentUtils::adjustBundle(PointCloud& pointCloud, std::vector<Pose>& cameraPoses, Intrinsics& intrinsics,
                                             const std::vector<Features>& image2dFeatures) {
     // dense numbering of the views that are actually observed (Ceres only knows blocks that appear in a residual)

@@ -93,6 +93,19 @@ def findCameraMatricesFromMatch(intrinsics: Intrinsics, matches, left: Features,
     return True, matches[m.reshape(-1) != 0].copy(), Pleft, Pright
 
 
+def findCameraMatricesFromMatch_gpu(intrinsics: Intrinsics, matches, left: Features, right: Features, ctx=None, seed=0):
+    """SfMStereoUtilities::findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) entirely on the device
+    (sfmb200_find_camera_matrices: five-point samples, scoring, OpenCV's sequential selection, recoverPose).
+    Returns (success, prunedMatches, Pleft, Pright) like the reference."""
+    ctx = ctx or default_context()
+    Pleft = np.eye(3, 4, dtype=np.float32)
+    E, R, t, _, pose_mask, s = ctx.find_camera_matrices(intrinsics.K, left.points, right.points, matches["queryIdx"], matches["trainIdx"], seed=seed)
+    if not s["found"]:
+        return False, matches[:0].copy(), Pleft, Pleft.copy()
+    Pright = np.concatenate([R, t.reshape(3, 1)], 1).astype(np.float32)           # :105-107
+    return True, matches[pose_mask != 0].copy(), Pleft, Pright
+
+
 def findCameraPoseFrom2D3DMatch(intrinsics: Intrinsics, points2D, points3D, ctx=None, iterations=100, seed=0):
     """SfMStereoUtilities::findCameraPoseFrom2D3DMatch (SfMStereoUtilities.cpp:208-243).  Returns (success, pose 3x4 float32)."""
     import cv2

@@ -1,7 +1,8 @@
 """BASELINE configs[0] (crazyhorse, 7 images) stage timing: the runSfM replay (sfm-toy-library_b200/runsfm.py) with the three
 hot-path stages on the GPU through the drop-in call shape, beside the same replay on the CPU (cv2 for matching and
 triangulation = the reference's own OpenCV calls, the oracle's Ceres restatement for adjustBundle).  RANSAC stages are
-cv2 in both arms (SURVEY.md 8 f-2).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
+cv2 in both arms (SURVEY.md 8 f-2); the gpu_batched_essential arm also runs findCameraMatricesFromMatch on the device
+(sfmb200_find_camera_matrices).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
 
     python tools/bench_cfg1.py [--reps 3] [--out gpurun_out/cfg1.json]
 """
@@ -17,8 +18,8 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 
 
-def run_arm(cfg1, arm, ctx=None, batched=True, threads=None):
-    from sfm_toy_library_b200 import runsfm, stages
+def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False):
+    from sfm_toy_library_b200 import ransac, runsfm, stages
     kw = {}
     if arm == "gpu":
         kw = dict(matchFeatures=lambda a, b: stages.matchFeatures(a, b, ctx=ctx),
@@ -26,6 +27,8 @@ def run_arm(cfg1, arm, ctx=None, batched=True, threads=None):
                   adjustBundle=lambda *a: stages.adjustBundle(*a, ctx=ctx))
         if batched:
             kw["matchAllPairs"] = lambda feats, pairs: stages.matchAllPairs(feats, pairs, ctx=ctx)
+        if essential:
+            kw["findCameraMatricesFromMatch"] = lambda *a: ransac.findCameraMatricesFromMatch_gpu(*a, ctx=ctx)
     else:
         import cv2
         from oracle import cv2_stages
@@ -52,6 +55,10 @@ def measure(reps=3):
     for name, kw in (("gpu_batched", dict(batched=True)), ("gpu_per_call", dict(batched=False))):
         runs = [run_arm(cfg1, "gpu", ctx, **kw) for _ in range(reps)]
         out[name] = min(runs, key=lambda r: r["hot_path_s"])
+    run_arm(cfg1, "gpu", ctx, essential=True)
+    runs = [run_arm(cfg1, "gpu", ctx, essential=True) for _ in range(reps)]
+    out["gpu_batched_essential"] = min(runs, key=lambda r: r["seconds"]["essential"])
+    out["essential_s"] = {"gpu_batched": out["gpu_batched"]["seconds"]["essential"], "gpu_batched_essential": out["gpu_batched_essential"]["seconds"]["essential"]}
     os.environ["SFMB200_MATCH_CACHE"] = "0"
     runs = [run_arm(cfg1, "gpu", ctx, batched=False) for _ in range(reps)]
     out["gpu_per_call_nocache"] = min(runs, key=lambda r: r["hot_path_s"])

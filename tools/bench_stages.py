@@ -140,7 +140,57 @@ def measure_triangulate(ctx, stream, flush, points=1_000_000, reps=5):
                              "sample": f"cv2 replay of triangulateViews on the first {ns} points (cv::triangulatePoints is serial)"}}
 
 
-def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None):
+def card():
+    """name and power limit of the card the numbers were measured on"""
+    import subprocess
+    import torch
+    try:
+        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
+                            timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        pl = "unknown"
+    return torch.cuda.get_device_name(0), pl
+
+
+def measure_essential(ctx, reps=20):
+    """findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) on the 21 crazyhorse pairs of tests/golden/cfg1_crazyhorse.npz:
+    sfmb200_find_camera_matrices (host clock around the synchronised call, warmed up, median over reps per pair) against
+    cv2.findEssentialMat(RANSAC, 0.999, 1 px) + cv2.recoverPose on one thread and on all threads."""
+    import cv2
+    g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
+    K = np.array([[2500, 0, 512], [0, 2500, 384], [0, 0, 1]], np.float32)
+    pairs = []
+    for p, (i, j) in enumerate(g["pairs"]):
+        a = g[f"pts_{int(i)}"][g[f"match_{p}_q"]]; b = g[f"pts_{int(j)}"][g[f"match_{p}_t"]]
+        pairs.append((np.ascontiguousarray(a), np.ascontiguousarray(b)))
+    gpu = []
+    for a, b in pairs:
+        ctx.find_camera_matrices(K, a, b)
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter(); ctx.find_camera_matrices(K, a, b); ts.append(time.perf_counter() - t0)
+        gpu.append(1e3 * float(np.median(ts)))
+
+    def cv_ms(threads):
+        cv2.setNumThreads(threads)
+        out = []
+        for a, b in pairs:
+            t0 = time.perf_counter()
+            E, m = cv2.findEssentialMat(a, b, 2500.0, (512.0, 384.0), cv2.RANSAC, 0.999, 1.0)
+            cv2.recoverPose(E[:3], a, b, focal=2500.0, pp=(512.0, 384.0), mask=m)
+            out.append(1e3 * (time.perf_counter() - t0))
+        return out
+    one = cv_ms(1); allt = cv_ms(os.cpu_count() or 1)
+    cv2.setNumThreads(-1)
+    name, pl = card()
+    return {"metric": "essential_ransac_pose_ms_per_call", "gpu_median_ms": float(np.median(gpu)), "gpu_max_ms": float(np.max(gpu)),
+            "cv2_1thread_median_ms": float(np.median(one)), "cv2_all_threads_median_ms": float(np.median(allt)),
+            "speedup_vs_cv2_1thread": float(np.median(one) / np.median(gpu)), "pairs": len(pairs), "matches": [int(len(a)) for a, _ in pairs],
+            "card": name, "power_limit": pl, "cpu_threads": os.cpu_count(),
+            "detail": {"gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt}}
+
+
+def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential")):
     import torch
     from sfm_toy_library_b200 import capi
     own = ctx is None
@@ -148,8 +198,13 @@ def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None):
         torch.cuda.set_device(0); ctx = capi.Context(0)
     stream = torch.cuda.ExternalStream(ctx.stream)
     flush = torch.empty(192 << 20, dtype=torch.uint8, device="cuda")
-    out = [measure_match(ctx, stream, flush, images, features, reps, "hamming"), measure_match(ctx, stream, flush, images, features, reps, "l2"),
-           measure_triangulate(ctx, stream, flush, points, reps)]
+    out = []
+    if "match" in stages:
+        out += [measure_match(ctx, stream, flush, images, features, reps, "hamming"), measure_match(ctx, stream, flush, images, features, reps, "l2")]
+    if "triangulate" in stages:
+        out.append(measure_triangulate(ctx, stream, flush, points, reps))
+    if "essential" in stages:
+        out.append(measure_essential(ctx))
     if own:
         ctx.close()
     return out
@@ -161,8 +216,9 @@ def main():
     ap.add_argument("--features", type=int, default=5000)
     ap.add_argument("--points", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential")
     args = ap.parse_args()
-    for line in measure_all(args.images, args.features, args.points, args.reps):
+    for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(",")):
         print(json.dumps(line), flush=True)
 
 
