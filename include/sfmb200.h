@@ -281,6 +281,53 @@ int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* 
 int sfmb200_five_point(sfmb200_ctx* ctx, const double* x1, const double* x2, int ns, double* E, int32_t* nsol);
 int sfmb200_essential_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, int32_t* nsol, int32_t* counts);
 
+/* ---- f-2: homography RANSAC for many image pairs, all on the device -------------------------------------------- */
+/*
+ * findHomographyInliers (SfMStereoUtilities.cpp:51-72) for every pair of a batch in one call:
+ *     H = findHomography(left, right, RANSAC, threshold_px, mask, max_iters, confidence);  count = countNonZero(mask)
+ * Identical to OpenCV 4.x (checked against cv2 4.13):
+ *   - the samples: cv::RNG seeded with (uint64)-1 at the start of every pair, getSubset's redraws of repeated indices and of quads
+ *     that fail the collinearity or orientation checks, so the same quads in the same order;
+ *   - the inlier test (float transfer error with H cast to float, err <= (float)(threshold^2)), the selection (a model replaces
+ *     the best only with more than max(best, 3) inliers) and RANSACUpdateNumIters(confidence, outlier ratio, 4, budget);
+ *   - hence the RANSAC inlier set, ransac_inliers and iterations;
+ *   - the returned mask and n_inliers: the inliers of the refined H, as cv::findHomography returns them.
+ * Not bit-identical: H itself.  The 4-point and least-squares DLT (normalised, eigenvector of the smallest eigenvalue of L^T L by
+ * cyclic Jacobi) and the Levenberg-Marquardt refinement (LMSolverImpl's schedule, 8 x 8 solves by Gaussian elimination) agree with
+ * OpenCV's to rounding, about 1e-7 of max|H| at worst on the crazyhorse pairs.  A point whose error lies within that rounding of the
+ * threshold could in principle flip; on those pairs the closest point is 1e-3 threshold^2 away.
+ * n == 4 follows findHomography: the DLT of the four points, no checks, no refinement, mask all ones.  n < 4 or no model: found = 0,
+ * n_inliers = 0, H and mask zero (the reference's `homography.empty()` branch).
+ *   pts [img_off[n_img] * 2]   key points of all images; image i owns pts[2 img_off[i] .. 2 img_off[i+1]); img_off [n_img + 1] monotone
+ *   pairs [n_pairs * 2]        (left image, right image)
+ *   match_q / match_t          per match, the key point index in the left / right image; pair p owns matches match_off[p] ..
+ *                              match_off[p+1]; match_off [n_pairs + 1], match_off[0] = 0, monotone
+ *   H [n_pairs * 9]            row-major, h22 = 1; may be NULL.  mask [match_off[n_pairs]]: may be NULL.  summary [n_pairs]: may be NULL.
+ * One CTA per pair, one host synchronisation per call.  Same inputs: bitwise-identical outputs, whether a pair is alone in a call or
+ * batched with others.  There is no seed: reproducing OpenCV's sample sequence is the point.
+ */
+typedef struct {
+    int max_iters;            /* 2000  cv::findHomography default; >= 1 */
+    double confidence;        /* 0.995 cv::findHomography default; in (0, 1) */
+    double threshold_px;      /* 10    RANSAC_THRESHOLD (SfMStereoUtilities.cpp:41); > 0 */
+    int refine_iters;         /* 10    Levenberg-Marquardt iterations of cv::findHomography; >= 1 */
+    int record_trace;         /* 0     1: keep every visited sample for sfmb200_homography_last_trace (20 bytes x max_iters per pair) */
+} sfmb200_homography_options;
+typedef struct {
+    int found;                /* 1: a model (cv::findHomography returned a non-empty H) */
+    int n_inliers;            /* countNonZero(mask): inliers of the refined H */
+    int ransac_inliers;       /* inliers of the best RANSAC model, before the refinement */
+    int iterations;           /* samples the sequential loop visited */
+} sfmb200_homography_summary;
+void sfmb200_homography_default_options(sfmb200_homography_options* opt);
+int sfmb200_find_homography_pairs(sfmb200_ctx* ctx, const float* pts, const int32_t* img_off, int n_img, const int32_t* pairs, int n_pairs,
+                                  const int32_t* match_q, const int32_t* match_t, const int64_t* match_off,
+                                  const sfmb200_homography_options* opt, double* H, uint8_t* mask, sfmb200_homography_summary* summary);
+/* Test hook: the samples the last sfmb200_find_homography_pairs call with record_trace = 1 visited for pair `pair`, in order: quads
+ * [cap][4] (indices into the pair's matches) and RANSAC inlier counts [cap] (-1: the DLT gave no model), the first min(cap, visited).
+ * Either output may be NULL.  Returns the number visited, or -1 (bad arguments, or no trace recorded). */
+int sfmb200_homography_last_trace(sfmb200_ctx* ctx, int pair, int cap, int32_t* quads, int32_t* counts);
+
 /* ---- f-3 ("next" row of SURVEY.md 8): ORB feature extraction, the step before matching ------------------------ */
 /*
  * SfM2DFeatureUtilities::extractFeatures (SfMToyLib/SfM2DFeatureUtilities.h:41-42, .cpp:46-51):

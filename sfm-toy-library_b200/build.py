@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libsfmb200.so")
-SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "orb.cu"]
+SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "homography.cu", "orb.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
@@ -94,6 +94,21 @@ def build_host_essential(force=False):
     return out
 
 
+def build_host_homography(force=False):
+    """The shim built with SFMB200_SHIM_HOMOGRAPHY (findHomographyInliers on the device too) + its test binary."""
+    hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_homography")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_homography.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    if force or _stale(out, deps):
+        r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", "-DSFMB200_SHIM_HOMOGRAPHY", os.path.join(hdir, "shim.cpp"),
+                            os.path.join(hdir, "test_shim_homography.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
+                            "-lpthread", "-o", out], capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("host shim (SFMB200_SHIM_HOMOGRAPHY) build failed")
+    return out
+
+
 def build_glue(force=False):
     """Host glue of SURVEY.md 8(f-1) (host/sfm_glue.cpp: indexed find2D3DMatches / mergeNewPointCloud) + its test binary, which
     checks it against the naive restatement in oracle/host_glue_naive.hpp.  Pure C++, no GPU, no CUDA library."""
@@ -128,5 +143,6 @@ if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
     print(build_host(force="--force" in sys.argv))
     print(build_host_essential(force="--force" in sys.argv))
+    print(build_host_homography(force="--force" in sys.argv))
     print(build_glue(force="--force" in sys.argv))
     print(build_ply(force="--force" in sys.argv))

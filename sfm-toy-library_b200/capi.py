@@ -61,6 +61,15 @@ class EssentialSummary(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class HomographyOptions(C.Structure):
+    _fields_ = [("max_iters", C.c_int), ("confidence", C.c_double), ("threshold_px", C.c_double), ("refine_iters", C.c_int),
+                ("record_trace", C.c_int)]
+
+
+class HomographySummary(C.Structure):
+    _fields_ = [("found", C.c_int), ("n_inliers", C.c_int), ("ransac_inliers", C.c_int), ("iterations", C.c_int)]
+
+
 def lib():
     """Load libsfmb200.so (built by build.py / __graft_entry__.build()).  No fallback."""
     global _lib
@@ -256,6 +265,42 @@ class Context:
             raise SfmB200Error("sfmb200_essential_last_trace failed")
         return smp[:S], n[:S], c[:int(n[:S].sum())]
 
+    # ------------------------------------------------------------------ f-2 homography RANSAC for many pairs
+    def find_homography_pairs(self, points, pairs, match_q, match_t, match_off, options=None, **kw):
+        """sfmb200_find_homography_pairs: cv::findHomography(RANSAC) for every pair in one call.  points: list of [n_i, 2] key
+        points per image; pairs [P, 2]; match_q / match_t: all pairs' matches concatenated, pair p owning match_off[p]:match_off[p+1].
+        options: HomographyOptions or keyword overrides of the defaults (max_iters, confidence, threshold_px, refine_iters,
+        record_trace).  Returns (H [P, 3, 3], mask [sum of matches] uint8, summary dict of arrays found / n_inliers /
+        ransac_inliers / iterations [P])."""
+        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
+        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
+        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
+        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
+        moff = np.ascontiguousarray(match_off, np.int64)
+        P = pairs.shape[0]
+        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
+            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+        o = options or homography_default_options(**kw)
+        H = np.zeros((max(P, 1), 9)); mask = np.zeros(max(mq.shape[0], 1), np.uint8); s = (HomographySummary * max(P, 1))()
+        self._check(lib().sfmb200_find_homography_pairs(self._h, _p(allp, C.c_float), _p(img_off, C.c_int32), len(pts), _p(pairs, C.c_int32), P,
+                                                        _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64), C.byref(o), _p(H, C.c_double),
+                                                        _p(mask, C.c_uint8), s))
+        summ = {k: np.array([getattr(s[p], k) for p in range(P)], np.int32) for k, _ in HomographySummary._fields_}
+        return H[:P].reshape(P, 3, 3), mask[:mq.shape[0]], summ
+
+    def homography_last_trace(self, pair):
+        """sfmb200_homography_last_trace: (quads [V, 4], RANSAC counts [V]) visited for `pair` by the last find_homography_pairs call
+        made with record_trace=1."""
+        f = lib().sfmb200_homography_last_trace
+        V = f(self._h, int(pair), 0, None, None)
+        if V < 0:
+            raise SfmB200Error("sfmb200_homography_last_trace failed (no trace recorded?)")
+        q = np.zeros((max(V, 1), 4), np.int32); c = np.zeros(max(V, 1), np.int32)
+        if f(self._h, int(pair), V, _p(q, C.c_int32), _p(c, C.c_int32)) != V:
+            raise SfmB200Error("sfmb200_homography_last_trace failed")
+        return q[:V], c[:V]
+
     # ------------------------------------------------------------------ f-3 ORB extraction
     def orb_detect_and_compute(self, images, nfeatures=5000, capacity=None):
         """sfmb200_orb_detect_and_compute[_batch]: `ORB::create(nfeatures)->detectAndCompute` (SfM2DFeatureUtilities.cpp:39, 48).
@@ -369,6 +414,14 @@ def ba_default_options(**kw):
 def essential_default_options(**kw):
     o = EssentialOptions()
     lib().sfmb200_essential_default_options(C.byref(o))
+    for k, v in kw.items():
+        setattr(o, k, v)
+    return o
+
+
+def homography_default_options(**kw):
+    o = HomographyOptions()
+    lib().sfmb200_homography_default_options(C.byref(o))
     for k, v in kw.items():
         setattr(o, k, v)
     return o

@@ -122,6 +122,9 @@ struct sfmb200_ctx {
     int rank = 0, nranks = 1;
     DevBuf ess_trace;           // samples / solution counts / inlier counts of the last essential-matrix RANSAC (essential.cu)
     int ess_trace_samples = 0;
+    DevBuf hg_trace;            // visited samples / counts of the last homography RANSAC with record_trace (homography.cu)
+    int hg_trace_pairs = 0, hg_trace_stride = 0;
+    std::vector<int32_t> hg_trace_visited;
 };
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);

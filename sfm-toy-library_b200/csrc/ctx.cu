@@ -55,6 +55,7 @@ void sfmb200_destroy(sfmb200_ctx* ctx) {
     for (auto& ev : ctx->orb_ev) if (ev) cudaEventDestroy(ev);
     ctx->scratch.release(); ctx->scratch2.release(); ctx->pinned.release(); ctx->ba_ws.release(); ctx->mcache.release(); ctx->ds_ws.release();
     ctx->ess_trace.release();
+    ctx->hg_trace.release();
     cudaStreamDestroy(ctx->stream);
     delete ctx;
 }

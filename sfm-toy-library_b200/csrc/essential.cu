@@ -96,18 +96,6 @@ essential_score_kernel(const float* __restrict__ a, const float* __restrict__ b,
     }
 }
 
-// RANSACUpdateNumIters (OpenCV calib3d ptsetreg.cpp), cvRound = round half to even
-__device__ int ransac_update_num_iters(double p, double ep, int model_points, int max_iters) {
-    p = fmin(fmax(p, 0.0), 1.0);
-    ep = fmin(fmax(ep, 0.0), 1.0);
-    double num = fmax(1.0 - p, DBL_MIN);
-    double denom = 1.0 - pow(1.0 - ep, (double)model_points);
-    if (denom < DBL_MIN) return 0;
-    num = log(num);
-    denom = log(denom);
-    return denom >= 0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
-}
-
 __global__ void __launch_bounds__(32)
 essential_select_kernel(const int32_t* __restrict__ nsol, const int32_t* __restrict__ counts, const Model* __restrict__ hyp, int S, int n,
                         int max_iters, double confidence, EssResult* __restrict__ res, double* __restrict__ cand, int32_t* __restrict__ cnt4) {

@@ -1,7 +1,10 @@
 // ransac_score.cuh -- the RANSAC error formulas, inlier rule and scoring / best / mask kernels of ransac.cu, shared with the
-// essential-matrix RANSAC (essential.cu), which scores its device-made hypotheses with the very same arithmetic.
+// essential-matrix and homography RANSACs (essential.cu, homography.cu), which score their device-made hypotheses with the very
+// same arithmetic, together with the sample budget of OpenCV's sequential loop.
 // See ransac.cu for which OpenCV computeError callback each formula mirrors.
 #pragma once
+#include <cfloat>
+#include <cmath>
 #include "common.cuh"
 
 namespace {
@@ -99,6 +102,18 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_mask_kernel(const float* __
 #pragma unroll
     for (int k = 0; k < 9; ++k) A[k] = aux[k];
     mask[i] = is_inlier<MODEL>(M, A, a, b, i, t2) ? 1 : 0;
+}
+
+// RANSACUpdateNumIters (OpenCV calib3d ptsetreg.cpp), cvRound = round half to even
+__device__ int ransac_update_num_iters(double p, double ep, int model_points, int max_iters) {
+    p = fmin(fmax(p, 0.0), 1.0);
+    ep = fmin(fmax(ep, 0.0), 1.0);
+    double num = fmax(1.0 - p, DBL_MIN);
+    double denom = 1.0 - pow(1.0 - ep, (double)model_points);
+    if (denom < DBL_MIN) return 0;
+    num = log(num);
+    denom = log(denom);
+    return denom >= 0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
 }
 
 }  // namespace

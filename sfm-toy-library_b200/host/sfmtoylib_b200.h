@@ -40,6 +40,7 @@ public:
 
 class SfMStereoUtilities {
 public:
+    static int findHomographyInliers(const Features& left, const Features& right, const Matching& matches);
     static bool findCameraMatricesFromMatch(const Intrinsics& intrinsics, const Matching& featureMatching, const Features& featuresLeft,
                                             const Features& featuresRight, Matching& prunedMatches, cv::Matx34f& Pleft, cv::Matx34f& Pright);
     static bool triangulateViews(const Intrinsics& intrinsics, const ImagePair imagePair, const Matching& matches,

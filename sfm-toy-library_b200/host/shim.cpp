@@ -173,6 +173,30 @@ bool SfMStereoUtilities::findCameraMatricesFromMatch(const Intrinsics& intrinsic
 }
 #endif  // SFMB200_SHIM_ESSENTIAL
 
+#ifdef SFMB200_SHIM_HOMOGRAPHY     // define it to replace findHomographyInliers (OpenCV's findHomography(RANSAC)) too
+// SfMStereoUtilities.cpp:51-72: cv::findHomography(RANSAC, RANSAC_THRESHOLD) -> countNonZero(mask), one device call
+// (sfmb200_find_homography_pairs with one pair); the count is OpenCV's.  0 for fewer than 4 matches or no model.
+int SfMStereoUtilities::findHomographyInliers(const Features& left, const Features& right, const Matching& matches) {
+    const int m = (int)matches.size();
+    if (m < 4) return 0;
+    std::vector<float> pts(2 * (left.points.size() + right.points.size()));
+    std::memcpy(pts.data(), left.points.data(), 2 * sizeof(float) * left.points.size());
+    std::memcpy(pts.data() + 2 * left.points.size(), right.points.data(), 2 * sizeof(float) * right.points.size());
+    const int32_t img_off[3] = {0, (int32_t)left.points.size(), (int32_t)(left.points.size() + right.points.size())};
+    const int32_t pair[2] = {0, 1};
+    const int64_t match_off[2] = {0, m};
+    std::vector<int32_t> mq(m), mt(m);
+    for (int i = 0; i < m; ++i) { mq[i] = matches[i].queryIdx; mt[i] = matches[i].trainIdx; }
+    sfmb200_homography_options opt;
+    sfmb200_homography_default_options(&opt);
+    opt.threshold_px = 10.0;                                                            // RANSAC_THRESHOLD, SfMStereoUtilities.cpp:41
+    sfmb200_homography_summary summary;
+    check(sfmb200_find_homography_pairs(context(), pts.data(), img_off, 2, pair, 1, mq.data(), mt.data(), match_off, &opt, nullptr, nullptr, &summary),
+          "sfmb200_find_homography_pairs");
+    return summary.found ? summary.n_inliers : 0;
+}
+#endif  // SFMB200_SHIM_HOMOGRAPHY
+
 void SfMBundleAdjustmentUtils::adjustBundle(PointCloud& pointCloud, std::vector<Pose>& cameraPoses, Intrinsics& intrinsics,
                                             const std::vector<Features>& image2dFeatures) {
     // dense numbering of the views that are actually observed (Ceres only knows blocks that appear in a residual)

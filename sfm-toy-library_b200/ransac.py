@@ -72,6 +72,26 @@ def findHomographyInliers(left: Features, right: Features, matches, ctx=None, it
     return int(counts[best])
 
 
+def homographyInliersAllPairs(features, pairs, matches, ctx=None):
+    """findHomographyInliers (SfMStereoUtilities.cpp:51-72) for every pair in one device call (sfmb200_find_homography_pairs):
+    cv::findHomography(RANSAC, RANSAC_THRESHOLD)'s own sample sequence, selection and refinement, so the counts are the
+    reference's.  features: per image Features; pairs [(i, j), ...]; matches: per pair a structured array with queryIdx / trainIdx.
+    Returns the inlier counts [len(pairs)] (0 for fewer than 4 matches or no model)."""
+    ctx = ctx or default_context()
+    if len(pairs) == 0:
+        return np.zeros(0, np.int64)
+    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
+    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
+    _, _, s = ctx.find_homography_pairs([f.points for f in features], pairs, mq, mt, off, threshold_px=RANSAC_THRESHOLD)
+    return np.where(s["found"] != 0, s["n_inliers"], 0).astype(np.int64)
+
+
+def findHomographyInliers_gpu(left: Features, right: Features, matches, ctx=None):
+    """SfMStereoUtilities::findHomographyInliers (SfMStereoUtilities.cpp:51-72) on the device: countNonZero of the mask
+    cv::findHomography(RANSAC, RANSAC_THRESHOLD) returns, 0 for fewer than 4 matches or no model."""
+    return int(homographyInliersAllPairs([left, right], [(0, 1)], [matches], ctx)[0])
+
+
 def findCameraMatricesFromMatch(intrinsics: Intrinsics, matches, left: Features, right: Features, ctx=None, iterations=200, seed=0):
     """SfMStereoUtilities::findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118).  Returns (success, prunedMatches, Pleft, Pright)."""
     import cv2

@@ -2,7 +2,8 @@
 hot-path stages on the GPU through the drop-in call shape, beside the same replay on the CPU (cv2 for matching and
 triangulation = the reference's own OpenCV calls, the oracle's Ceres restatement for adjustBundle).  RANSAC stages are
 cv2 in both arms (SURVEY.md 8 f-2); the gpu_batched_essential arm also runs findCameraMatricesFromMatch on the device
-(sfmb200_find_camera_matrices).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
+(sfmb200_find_camera_matrices), the gpu_batched_homography arm the homography inliers of all pairs in one device call
+(sfmb200_find_homography_pairs).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
 
     python tools/bench_cfg1.py [--reps 3] [--out gpurun_out/cfg1.json]
 """
@@ -18,7 +19,7 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 
 
-def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False):
+def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, homography=False):
     from sfm_toy_library_b200 import ransac, runsfm, stages
     kw = {}
     if arm == "gpu":
@@ -29,6 +30,8 @@ def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False):
             kw["matchAllPairs"] = lambda feats, pairs: stages.matchAllPairs(feats, pairs, ctx=ctx)
         if essential:
             kw["findCameraMatricesFromMatch"] = lambda *a: ransac.findCameraMatricesFromMatch_gpu(*a, ctx=ctx)
+        if homography:
+            kw["homographyInliersAllPairs"] = lambda f, pr, m: ransac.homographyInliersAllPairs(f, pr, m, ctx=ctx)
     else:
         import cv2
         from oracle import cv2_stages
@@ -59,6 +62,11 @@ def measure(reps=3):
     runs = [run_arm(cfg1, "gpu", ctx, essential=True) for _ in range(reps)]
     out["gpu_batched_essential"] = min(runs, key=lambda r: r["seconds"]["essential"])
     out["essential_s"] = {"gpu_batched": out["gpu_batched"]["seconds"]["essential"], "gpu_batched_essential": out["gpu_batched_essential"]["seconds"]["essential"]}
+    run_arm(cfg1, "gpu", ctx, homography=True)
+    runs = [run_arm(cfg1, "gpu", ctx, homography=True) for _ in range(reps)]
+    out["gpu_batched_homography"] = min(runs, key=lambda r: r["seconds"]["homography"])
+    out["homography_s"] = {"gpu_batched": out["gpu_batched"]["seconds"]["homography"],
+                           "gpu_batched_homography": out["gpu_batched_homography"]["seconds"]["homography"]}
     os.environ["SFMB200_MATCH_CACHE"] = "0"
     runs = [run_arm(cfg1, "gpu", ctx, batched=False) for _ in range(reps)]
     out["gpu_per_call_nocache"] = min(runs, key=lambda r: r["hot_path_s"])

@@ -190,6 +190,81 @@ def measure_essential(ctx, reps=20):
             "detail": {"gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt}}
 
 
+def synthetic_homography_set(images=50, seed=0):
+    """Seeded all-pairs set: per pair a planar scene of 200-1200 matches at 30-70 % outliers, its points appended to the two images."""
+    rs = np.random.RandomState(seed)
+    pts = [[] for _ in range(images)]; sizes = [0] * images
+    pairs, mq, mt, off = [], [], [], [0]
+    for i in range(images):
+        for j in range(i + 1, images):
+            n = int(rs.randint(200, 1201)); r = rs.uniform(0.3, 0.7)
+            H = np.eye(3) + np.r_[rs.normal(0, 0.08, 6), rs.normal(0, 1e-4, 2), 0].reshape(3, 3)
+            a = np.c_[rs.uniform(0, 1024, n), rs.uniform(0, 768, n)]
+            ph = np.c_[a, np.ones(n)] @ H.T
+            b = ph[:, :2] / ph[:, 2:] + rs.normal(0, 0.5, (n, 2))
+            k = int(r * n); o = rs.choice(n, k, replace=False); b[o] = np.c_[rs.uniform(0, 1024, k), rs.uniform(0, 768, k)]
+            pts[i].append(a.astype(np.float32)); pts[j].append(b.astype(np.float32))
+            mq.append(np.arange(n, dtype=np.int32) + sizes[i]); mt.append(np.arange(n, dtype=np.int32) + sizes[j])
+            sizes[i] += n; sizes[j] += n
+            pairs.append((i, j)); off.append(off[-1] + n)
+    return [np.concatenate(p) for p in pts], np.array(pairs, np.int32), np.concatenate(mq), np.concatenate(mt), np.array(off, np.int64)
+
+
+def measure_homography(ctx, images=50, reps=3):
+    """findHomographyInliers (SfMStereoUtilities.cpp:51-72): sfmb200_find_homography_pairs, host clock around the synchronised
+    call (warmed up; median and max over reps), on the 21 crazyhorse pairs one call per pair and all in one call, and on a seeded
+    synthetic 50-image set (1225 pairs) in one call; cv2.findHomography(RANSAC, 10) on one host thread for the same work; the
+    kernel time of the batched calls from torch.profiler in a separate pass."""
+    import cv2
+    import torch
+    g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
+    feats = [g[f"pts_{i}"] for i in range(len(g["files"]))]
+    ch_pairs = np.array(g["pairs"], np.int32)
+    ch_q = [g[f"match_{p}_q"] for p in range(len(ch_pairs))]; ch_t = [g[f"match_{p}_t"] for p in range(len(ch_pairs))]
+    ch_off = np.zeros(len(ch_pairs) + 1, np.int64); ch_off[1:] = np.cumsum([len(q) for q in ch_q])
+    ch_q = np.concatenate(ch_q); ch_t = np.concatenate(ch_t)
+    sy = synthetic_homography_set(images)
+
+    def timed(fn):
+        fn()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter(); fn(); ts.append(1e3 * (time.perf_counter() - t0))
+        return ts
+    per_pair = []
+    for p in range(len(ch_pairs)):
+        sl = slice(int(ch_off[p]), int(ch_off[p + 1]))
+        per_pair.append(timed(lambda: ctx.find_homography_pairs(feats, ch_pairs[p:p + 1], ch_q[sl], ch_t[sl], np.array([0, sl.stop - sl.start]))))
+    batched = timed(lambda: ctx.find_homography_pairs(feats, ch_pairs, ch_q, ch_t, ch_off))
+    syn = timed(lambda: ctx.find_homography_pairs(*sy))
+
+    def cv_ms(points, pairs, q, t, off):
+        cv2.setNumThreads(1)
+        t0 = time.perf_counter()
+        for p, (i, j) in enumerate(pairs):
+            sl = slice(int(off[p]), int(off[p + 1]))
+            cv2.findHomography(points[i][q[sl]], points[j][t[sl]], cv2.RANSAC, 10.0)
+        cv2.setNumThreads(-1)
+        return 1e3 * (time.perf_counter() - t0)
+    cv_ch = cv_ms(feats, ch_pairs, ch_q, ch_t, ch_off); cv_syn = cv_ms(*sy)
+    kernel = {}
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        ctx.find_homography_pairs(feats, ch_pairs, ch_q, ch_t, ch_off)
+        ctx.find_homography_pairs(*sy)
+    for e in prof.events():
+        if "homography_pairs_kernel" in e.name:
+            kernel.setdefault("crazyhorse_21" if not kernel else "synthetic_1225", 1e-3 * e.device_time_total)
+    name, pl = card()
+    med = [float(np.median(x)) for x in per_pair]
+    return {"metric": "homography_ransac_ms_per_call", "card": name, "power_limit": pl,
+            "crazyhorse_per_pair_median_ms": float(np.median(med)), "crazyhorse_per_pair_max_ms": float(np.max([max(x) for x in per_pair])),
+            "crazyhorse_per_pair_sum_of_medians_ms": float(np.sum(med)),
+            "crazyhorse_21_one_call_median_ms": float(np.median(batched)), "crazyhorse_21_one_call_max_ms": float(np.max(batched)),
+            "synthetic_1225_one_call_median_ms": float(np.median(syn)), "synthetic_1225_one_call_max_ms": float(np.max(syn)),
+            "synthetic_matches": int(sy[4][-1]), "cv2_1thread_crazyhorse_21_ms": cv_ch, "cv2_1thread_synthetic_1225_ms": cv_syn,
+            "kernel_ms_torch_profiler": kernel}
+
+
 def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential")):
     import torch
     from sfm_toy_library_b200 import capi
@@ -205,6 +280,8 @@ def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, st
         out.append(measure_triangulate(ctx, stream, flush, points, reps))
     if "essential" in stages:
         out.append(measure_essential(ctx))
+    if "homography" in stages:
+        out.append(measure_homography(ctx, images))
     if own:
         ctx.close()
     return out
@@ -216,7 +293,7 @@ def main():
     ap.add_argument("--features", type=int, default=5000)
     ap.add_argument("--points", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential")
+    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography")
     args = ap.parse_args()
     for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(",")):
         print(json.dumps(line), flush=True)
