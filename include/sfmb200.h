@@ -338,7 +338,7 @@ int sfmb200_homography_last_trace(sfmb200_ctx* ctx, int pair, int cap, int32_t* 
  * HARRIS_SCORE, patchSize 31, fastThreshold 20).  Output is bit-identical to OpenCV's (cv2 4.13 in this image): the same key points
  * in the same order with the same pt / size / angle / response / octave, and the same 32-byte descriptors.
  *   image        8-bit pixels, channels = 1 (grey) or 3 (B,G,R interleaved; converted like cvtColor(COLOR_BGR2GRAY)); row_stride in
- *                bytes (0 = packed rows).  8 <= width, height <= 65535, width * height <= 2^28.  JPEG/PNG decoding stays with the caller (cv::imread).
+ *                bytes (0 = packed rows).  8 <= width, height <= 65535, width * height <= 2^28.  JPEG files decode with sfmb200_decode_jpeg_batch below.
  *   keypoints    [max_keypoints] records with the memory layout of cv::KeyPoint (28 bytes), so a shim can copy them straight into a
  *                std::vector<cv::KeyPoint>; class_id = -1.  KeyPointsToPoints (SfMCommon.cpp:89-94) is the x,y prefix of every record.
  *   descriptors  [max_keypoints * 32]
@@ -368,6 +368,34 @@ int sfmb200_orb_last_timings(const sfmb200_ctx* ctx, double* ms8);
 /* Self-test of the context's host thread pool (csrc/host_pool.h; staging and retainBest tasks of the ORB stage run on it): `rounds`
  * parallel loops of varying length on `n_threads` threads; returns a checksum >= 0, -1 on bad arguments, -2 on a wrong result. */
 int64_t sfmb200_host_pool_selftest(int n_threads, int rounds, int max_tasks);
+
+/* ---- f-3: JPEG decoding, the step before ORB extraction --------------------------------------------------------- */
+/*
+ * The imread loop of SfM::setImagesDirectory (SfM.cpp:123-135) for all images of a run in one call:  mImages.push_back(imread(file)).
+ * The output is byte-identical to cv::imread(file, IMREAD_COLOR) with the libjpeg-turbo 3.1 OpenCV 4.13 bundles: ISLOW integer IDCT,
+ * fancy upsampling, libjpeg's integer YCbCr -> RGB tables, B,G,R order, EXIF orientation (tag 0x0112 of IFD0 in the first APP1)
+ * applied -- orientations 5-8 swap width and height.  A grey file gives three equal channels.
+ * Supported: baseline and extended sequential Huffman JPEG (SOF0 / SOF1), 8-bit, 1 component or 3 (YCbCr) with the sampling
+ * cv::imencode writes (4:4:4, 4:2:2, 4:2:0, 4:4:0, 4:1:1), optimised or standard Huffman tables, restart intervals, any size, any
+ * APPn / COM segments.  Progressive, arithmetic-coded, lossless, 12-bit, 4-component and RGB (Adobe transform 0) files and other
+ * sampling factors return SFMB200_ERR_UNSUPPORTED.  Truncated or corrupt data returns SFMB200_ERR_INVALID -- unlike libjpeg, which
+ * warns, pads and returns an image.  sfmb200_last_error names the image and the reason; the context stays usable.
+ *
+ * sfmb200_jpeg_info: host only (no context, no GPU): the output size (after orientation) and the component count of the file, or the
+ * status a decode would return.
+ * sfmb200_decode_jpeg_batch: decodes the n files data[i] [size[i] bytes] into caller-owned host buffers out_bgr[i], rows of
+ * out_stride[i] bytes (out_stride NULL or 0 = packed rows, width * 3).  The images may differ in size.  One upload of all
+ * entropy-coded data, one download, one host synchronisation per call.  An image decodes to the same bytes alone or in a batch.  If
+ * any file fails, the call returns that status and the outputs are unspecified.  At most 65535 files and 512 MB of entropy-coded data
+ * per call.
+ * sfmb200_jpeg_last_stats: the Huffman phase of the last call: [0] subsequences of 1024 bits, [1] codewords decoded by the first pass,
+ * [2] codewords decoded again to synchronise, [3] parallel synchronisation rounds run, [4] subsequences the in-order sweep re-decoded,
+ * [5] bytes uploaded, [6] bytes downloaded.
+ */
+int sfmb200_jpeg_info(const uint8_t* data, size_t size, int* width, int* height, int* components);
+int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, uint8_t* const* out_bgr,
+                              const size_t* out_stride);
+int sfmb200_jpeg_last_stats(const sfmb200_ctx* ctx, int64_t* stats7);
 
 /* ---- multi-GPU plumbing (NCCL, one process per GPU) ------------------------------------------------------ */
 #define SFMB200_UNIQUE_ID_BYTES 128

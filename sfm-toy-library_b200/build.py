@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libsfmb200.so")
-SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "homography.cu", "orb.cu"]
+SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "homography.cu", "orb.cu", "jpeg.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
@@ -109,6 +109,21 @@ def build_host_homography(force=False):
     return out
 
 
+def build_images(force=False):
+    """sfmtoylib::readImages (host/sfm_images.cpp: the imread loop of setImagesDirectory over sfmb200_decode_jpeg_batch) + its driver."""
+    hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_images")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    deps = [os.path.join(hdir, f) for f in ("sfm_images.cpp", "sfm_images.h", "test_images.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    if force or _stale(out, deps):
+        r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", os.path.join(hdir, "sfm_images.cpp"), os.path.join(hdir, "test_images.cpp"),
+                            "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib", "-lpthread", "-o", out],
+                           capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("readImages build failed")
+    return out
+
+
 def build_glue(force=False):
     """Host glue of SURVEY.md 8(f-1) (host/sfm_glue.cpp: indexed find2D3DMatches / mergeNewPointCloud) + its test binary, which
     checks it against the naive restatement in oracle/host_glue_naive.hpp.  Pure C++, no GPU, no CUDA library."""
@@ -144,5 +159,6 @@ if __name__ == "__main__":
     print(build_host(force="--force" in sys.argv))
     print(build_host_essential(force="--force" in sys.argv))
     print(build_host_homography(force="--force" in sys.argv))
+    print(build_images(force="--force" in sys.argv))
     print(build_glue(force="--force" in sys.argv))
     print(build_ply(force="--force" in sys.argv))

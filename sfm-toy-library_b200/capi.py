@@ -360,6 +360,36 @@ class Context:
         self._check(lib().sfmb200_orb_download_level(self._h, int(stage), int(image), int(level), _p(out, C.c_uint8)))
         return out
 
+    # ------------------------------------------------------------------ f-3 JPEG decoding
+    @staticmethod
+    def jpeg_info(data):
+        """sfmb200_jpeg_info (host only): (status, width, height, components) of a JPEG file given as bytes."""
+        return jpeg_info(data)
+
+    def decode_jpeg(self, files):
+        """sfmb200_decode_jpeg_batch: `files` is a list of JPEG files as bytes; returns a list of uint8 [h, w, 3] B,G,R images,
+        byte-identical to cv2.imdecode(buf, IMREAD_COLOR), in one call.  Raises SfmB200Error (naming the file) if any file is
+        unsupported (status 5) or corrupt (status 1)."""
+        files = [bytes(f) for f in files]
+        n = len(files)
+        if n == 0:
+            return []
+        outs = []
+        for f in files:
+            rc, w, h, _ = jpeg_info(f)
+            outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
+        data = (C.c_char_p * n)(*files)
+        sizes = (C.c_size_t * n)(*[len(f) for f in files])
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        self._check(lib().sfmb200_decode_jpeg_batch(self._h, data, sizes, n, ptrs, None))
+        return outs
+
+    def jpeg_last_stats(self):
+        """Huffman-phase counters of the last decode_jpeg call (sfmb200_jpeg_last_stats)."""
+        s = np.zeros(7, np.int64)
+        self._check(lib().sfmb200_jpeg_last_stats(self._h, _p(s, C.c_int64)))
+        return dict(zip(("subsequences", "codewords_first_pass", "codewords_sync", "rounds", "swept", "upload_bytes", "download_bytes"), s.tolist()))
+
     # ------------------------------------------------------------------ multi-GPU
     def comm_init(self, unique_id, rank, nranks):
         buf = (C.c_uint8 * UNIQUE_ID_BYTES).from_buffer_copy(bytes(unique_id)) if unique_id is not None else None
@@ -393,6 +423,15 @@ def orb_retain_best(response, n_points):
     if n < 0:
         raise SfmB200Error("sfmb200_orb_retain_best: bad arguments")
     return order[:n].copy()
+
+
+def jpeg_info(data):
+    """sfmb200_jpeg_info: (status, width, height, components) of a JPEG file given as bytes, without a context or a GPU.  width and
+    height are the decoded image's (after EXIF orientation); status 0 = decodable, 1 = invalid, 5 = unsupported."""
+    data = bytes(data)
+    w = C.c_int(0); h = C.c_int(0); c = C.c_int(0)
+    rc = lib().sfmb200_jpeg_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(c))
+    return int(rc), w.value, h.value, c.value
 
 
 def comm_unique_id():

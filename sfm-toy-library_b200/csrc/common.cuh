@@ -125,6 +125,9 @@ struct sfmb200_ctx {
     DevBuf hg_trace;            // visited samples / counts of the last homography RANSAC with record_trace (homography.cu)
     int hg_trace_pairs = 0, hg_trace_stride = 0;
     std::vector<int32_t> hg_trace_visited;
+    DevBuf jpeg_dev;                    // JPEG decoding (jpeg.cu): tables, entropy data, coefficients, planes, images of the last batch
+    PinBuf jpeg_pin_up, jpeg_pin_down;  // its one upload and its one download
+    int64_t jpeg_stats[7] = {0, 0, 0, 0, 0, 0, 0};   // sfmb200_jpeg_last_stats of the last batch
 };
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);

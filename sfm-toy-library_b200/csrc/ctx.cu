@@ -56,6 +56,7 @@ void sfmb200_destroy(sfmb200_ctx* ctx) {
     ctx->scratch.release(); ctx->scratch2.release(); ctx->pinned.release(); ctx->ba_ws.release(); ctx->mcache.release(); ctx->ds_ws.release();
     ctx->ess_trace.release();
     ctx->hg_trace.release();
+    ctx->jpeg_dev.release(); ctx->jpeg_pin_up.release(); ctx->jpeg_pin_down.release();
     cudaStreamDestroy(ctx->stream);
     delete ctx;
 }

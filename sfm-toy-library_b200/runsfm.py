@@ -128,6 +128,30 @@ class SfM:
         sfm.seconds["extract"] = dt; sfm.calls["extract"] = len(images)
         return sfm
 
+    @classmethod
+    def from_directory(cls, path, readImages: Callable = None, extractAllFeatures: Callable = None, **kw):
+        """SfM::setImagesDirectory (SfM.cpp:97-139): the .jpg / .png files of `path` (extension compared case-insensitively), sorted
+        by name, read by the injected stage (default cv2.imread per file; stages.readImages decodes them all on the device), then
+        from_images.  The reference's optional downscale (:127-129) is not applied."""
+        import os
+        names = sorted(f for f in os.listdir(path) if os.path.splitext(f)[1].lower() in (".jpg", ".png"))
+        if not names:
+            raise ValueError(f"Unable to find valid files in images directory (\"{path}\").")
+        files = [os.path.join(path, f) for f in names]
+        t0 = time.perf_counter()
+        if readImages is None:
+            import cv2
+            images = [cv2.imread(f) for f in files]
+        else:
+            images = list(readImages(files))
+        dt = time.perf_counter() - t0
+        for f, im in zip(files, images):
+            if im is None or im.size == 0:
+                raise ValueError(f"Unable to read image from file: {f}")
+        sfm = cls.from_images(images, extractAllFeatures, **kw)
+        sfm.seconds["read"] = dt; sfm.calls["read"] = len(files)
+        return sfm
+
     # ---- timing helper
     def _timed(self, key, fn, *a, **kw):
         t0 = time.perf_counter()

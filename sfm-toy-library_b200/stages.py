@@ -64,6 +64,18 @@ def GetAlignedMatching(size):          # SfMCommon.cpp:120-126
     return m
 
 
+def readImages(files: List[str], ctx=None) -> List[np.ndarray]:
+    """The imread loop of SfM::setImagesDirectory (SfM.cpp:123-135) on the device: every file decoded in one
+    sfmb200_decode_jpeg_batch call, byte-identical to cv2.imread(file) (B,G,R, EXIF orientation applied).  Only JPEG files decode
+    (there is no host fallback): any other file raises capi.SfmB200Error naming it."""
+    ctx = ctx or default_context()
+    blobs = []
+    for f in files:
+        with open(f, "rb") as fh:
+            blobs.append(fh.read())
+    return ctx.decode_jpeg(blobs)
+
+
 ORB_FEATURES = 5000                    # mDetector = ORB::create(5000), SfM2DFeatureUtilities.cpp:39
 
 
