@@ -20,7 +20,7 @@
 //   * reduced system summed over ranks: peer-memory kernel (loads the peers' buffers over NVLink into a local summed copy)
 //     or one NCCL all-reduce (S, rhs, gradient, diag, cost in one buffer).
 //   * ba_assemble + chol.cuh (streaming dataflow tile Cholesky, rhs carried as an extra row so the forward substitution is
-//     free, staged back substitution with inverse diagonal tiles): K4.
+//     free, back substitution with inverse diagonal tiles on a CTA cluster or, for large n, one CTA): K4.
 //   * ba_backsub_eval_kernel (point-major, default): delta_p from Jacobians re-evaluated at x, candidate point, model cost
 //     change and candidate cost fused; ba_backsub_z_kernel (SFMB200_BA_BACKSUB=stored) reads the stored Z blocks instead.
 //   LM control runs on the DEVICE (LMState, ba_lm_control_kernel); the host enqueues chunks of iterations and reads the
@@ -1053,11 +1053,11 @@ struct sfmb200_ba_problem {
     double* locals;                   // [8] identical on every rank
     unsigned long long* gmax_pt_bits; int* fail;   // fail[0] point blocks, fail[1] dense Cholesky
     double* A; double* y_cf; double* dinv;
-    int grid_point = 0, grid_backsub = 0, grid_camera = 0; bool one_wave = true;   // persistent grids = co-resident CTA count
+    int grid_point = 0, grid_backsub = 0, grid_camera = 0;   // persistent grids = co-resident CTA count
     double* Linv = nullptr;           // [npad/NB][NB][NB] inverses of the diagonal tiles (dataflow Cholesky -> back substitution)
-    bool backsolve_staged = false, backsolve_cluster = false;
-    uint4* chol_ll = nullptr; int chol_grid_stream = 0; bool chol_stream = true;
-    unsigned* chol_ready = nullptr; unsigned chol_epoch = 0; int chol_grid = 0; bool chol_fused = true, chol_lookahead = false;   // dataflow Cholesky (K4)
+    bool backsolve_cluster = false;   // back substitution on a CTA cluster (small enough n) or on one CTA
+    uint4* chol_ll = nullptr; int chol_grid_stream = 0;
+    unsigned* chol_ready = nullptr; unsigned chol_epoch = 0;   // dataflow Cholesky (K4)
     unsigned* solve_counter = nullptr;   // device-side number of the current dense solve (incremented by ba_assemble_kernel)
     double* h_scal = nullptr;         // pinned read-back: sums[8] post[8] locals[8] gmax fail
     bool have_scale = false;
@@ -1126,9 +1126,7 @@ static size_t point_smem_bytes(int G, int maxk) {
 }
 
 // Grid for a grid-stride kernel: exactly the number of co-resident CTAs (one balanced wave), cached per problem.
-// SFMB200_BA_GRID=legacy keeps the fixed multiple of the SM count (A/B measurements).
-template <typename K> static int resident_grid(sfmb200_ba_problem* P, int* cache, K kernel, int threads, size_t smem, int work_blocks, int legacy_per_sm) {
-    if (!P->one_wave) return std::max(1, std::min(work_blocks, P->ctx->sm_count * legacy_per_sm));
+template <typename K> static int resident_grid(sfmb200_ba_problem* P, int* cache, K kernel, int threads, size_t smem, int work_blocks) {
     if (*cache == 0) {
         int per_sm = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) { cudaGetLastError(); per_sm = 1; }
@@ -1141,7 +1139,7 @@ template <int G> static int launch_point_pass(sfmb200_ba_problem* P, const BAVie
     sfmb200_ctx* ctx = P->ctx;
     const int GB = PT_THREADS / G;
     if (P->gather) {
-        const int blocks = resident_grid(P, &P->grid_point, ba_point_kernel<G, true>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
+        const int blocks = resident_grid(P, &P->grid_point, ba_point_kernel<G, true>, PT_THREADS, 0, ceil_div(P->np, GB));
         ba_point_kernel<G, true><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, inv_radius);
         SFM_LAUNCH_CHECK(ctx);
         return SFMB200_OK;
@@ -1167,19 +1165,19 @@ template <int G> static int launch_backsub(sfmb200_ba_problem* P, const BAView& 
     if (P->backsub_from_z) {            // gather mode: Z_o is in Zbuf, no Jacobian needed (inside the LM loop the radius comes from LMState)
         const size_t tab = sizeof(double) * 18 * (size_t)P->nc;
         if (tab <= 40 * 1024) {
-            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB), 16);
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB));
             ba_backsub_z_kernel<G, true><<<blocks, PT_THREADS, tab, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
         } else {
-            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB));
             ba_backsub_z_kernel<G, false><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
         }
     } else {                            // default: Jacobians re-evaluated at x (no Z blocks)
         const size_t tab = sizeof(BacksubCam) * (size_t)P->nc;
         if (tab <= 40 * 1024) {
-            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB), 16);
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB));
             ba_backsub_eval_kernel<G, true><<<blocks, PT_THREADS, tab, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
         } else {
-            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB), 16);
+            const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_eval_kernel<G, false>, PT_THREADS, 0, ceil_div(P->np, GB));
             ba_backsub_eval_kernel<G, false><<<blocks, PT_THREADS, 0, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
         }
     }
@@ -1289,7 +1287,7 @@ static int schur_pass(sfmb200_ba_problem* P, const sfmb200_ba_options* opt, doub
             ba_combine_kernel<<<P->nc + ceil_div(P->n_pairs_nonempty, COMBINE_THREADS / 32), COMBINE_THREADS, 0, ctx->stream>>>(v, ra, 0, nullptr, P->fpart, P->counters + 2); SFM_LAUNCH_CHECK(ctx);
         } else {
             if (es) SFM_CUDA(ctx, cudaEventRecord(es->ev[2], ctx->stream));
-            const int blocks = resident_grid(P, &P->grid_camera, ba_camera_kernel<false, false>, CAM_THREADS, 0, ceil_div(P->nobs, CAM_THREADS), 4);
+            const int blocks = resident_grid(P, &P->grid_camera, ba_camera_kernel<false, false>, CAM_THREADS, 0, ceil_div(P->nobs, CAM_THREADS));
             ba_camera_kernel<false, false><<<blocks, CAM_THREADS, 0, ctx->stream>>>(v, ceil_div(P->nobs, blocks), nullptr); SFM_LAUNCH_CHECK(ctx);
         }
         if (es) SFM_CUDA(ctx, cudaEventRecord(es->ev[3], ctx->stream));
@@ -1305,31 +1303,13 @@ static int dense_solve(sfmb200_ba_problem* P, const sfmb200_ba_options* opt, dou
     ba_assemble_kernel<<<dim3(ceil_div(npad, 128), npad), 128, 0, ctx->stream>>>(summed(P, P->Sblk), summed(P, P->Scf), summed(P, P->Sff), summed(P, P->rhs), summed(P, P->dcf), P->nc, npad, 1.0 / radius,
                                                                                  opt->min_lm_diagonal, opt->max_lm_diagonal, P->A, st, P->solve_counter);
     SFM_LAUNCH_CHECK(ctx);
-    if (P->chol_fused) {
-        const bool la = P->chol_lookahead || P->chol_stream;
-        const int ntasks = chol_fused_tasks(nbk, la);
-        const int grid = std::min(ntasks, P->chol_grid);
-        if (P->chol_stream) chol_stream_kernel<<<std::min(ntasks, P->chol_grid_stream), CS_THREADS, 0, ctx->stream>>>(P->A, npad, P->n, nbk, ntasks, P->dinv, P->fail + 1, P->chol_ready, P->chol_ll,
-                                                                                                                   0u, P->Linv, nullptr, skip, P->solve_counter);
-        else if (la) chol_fused_kernel<true><<<grid, PANEL_WARPS * 32, 0, ctx->stream>>>(P->A, npad, P->n, nbk, ntasks, P->dinv, P->fail + 1, P->chol_ready, 0u, P->Linv, nullptr, skip, P->solve_counter);
-        else chol_fused_kernel<false><<<grid, PANEL_WARPS * 32, 0, ctx->stream>>>(P->A, npad, P->n, nbk, ntasks, P->dinv, P->fail + 1, P->chol_ready, 0u, P->Linv, nullptr, skip, P->solve_counter);
-        SFM_LAUNCH_CHECK(ctx);
-    } else {
-        for (int k = 0; k < nbk; ++k) {
-            chol_panel_kernel<<<std::max(1, ceil_div(nbk - k - 1, PANEL_WARPS)), PANEL_WARPS * 32, 0, ctx->stream>>>(P->A, npad, P->n, k, nbk, P->dinv, P->fail + 1, skip); SFM_LAUNCH_CHECK(ctx);
-            const int T = nbk - k - 1;
-            if (T > 0) { chol_update_kernel<<<T * (T + 1) / 2, dim3(NB, NB), 0, ctx->stream>>>(P->A, npad, k, nbk, skip); SFM_LAUNCH_CHECK(ctx); }
-        }
-    }
-    {
-        const size_t smem = chol_backsolve_smem(npad, P->backsolve_staged);
-        if (P->backsolve_cluster) chol_backsolve_cluster_kernel<<<BS_CLUSTER, chol_backsolve_cluster_threads(P->n), chol_backsolve_cluster_smem(P->n), ctx->stream>>>(P->A, P->Linv, npad, P->n, P->y_cf, P->fail + 1, skip);
-        else if (P->backsolve_staged && P->chol_fused) chol_backsolve_kernel<true, true><<<1, 640, smem, ctx->stream>>>(P->A, P->dinv, P->Linv, npad, P->n, P->y_cf, skip);
-        else if (P->backsolve_staged) chol_backsolve_kernel<true, false><<<1, 640, smem, ctx->stream>>>(P->A, P->dinv, P->Linv, npad, P->n, P->y_cf, skip);
-        else if (P->chol_fused) chol_backsolve_kernel<false, true><<<1, 640, smem, ctx->stream>>>(P->A, P->dinv, P->Linv, npad, P->n, P->y_cf, skip);
-        else chol_backsolve_kernel<false, false><<<1, 640, smem, ctx->stream>>>(P->A, P->dinv, P->Linv, npad, P->n, P->y_cf, skip);
-        SFM_LAUNCH_CHECK(ctx);
-    }
+    const int ntasks = chol_stream_tasks(nbk);
+    chol_stream_kernel<<<std::min(ntasks, P->chol_grid_stream), CS_THREADS, 0, ctx->stream>>>(P->A, npad, P->n, nbk, ntasks, P->dinv, P->fail + 1, P->chol_ready, P->chol_ll,
+                                                                                          0u, P->Linv, nullptr, skip, P->solve_counter);
+    SFM_LAUNCH_CHECK(ctx);
+    if (P->backsolve_cluster) chol_backsolve_cluster_kernel<<<BS_CLUSTER, chol_backsolve_cluster_threads(P->n), chol_backsolve_cluster_smem(P->n), ctx->stream>>>(P->A, P->Linv, npad, P->n, P->y_cf, P->fail + 1, skip);
+    else chol_backsolve_kernel<<<1, 640, chol_backsolve_smem(npad), ctx->stream>>>(P->A, P->Linv, npad, P->n, P->y_cf, skip);
+    SFM_LAUNCH_CHECK(ctx);
     return SFMB200_OK;
 }
 
@@ -1483,36 +1463,16 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         CRT(cudaMemsetAsync(P->chol_ready, 0, 4 * (size_t)nbk * nbk, st));
         CRT(cudaMemsetAsync(P->chol_ll, 0, chol_ll_bytes(nbk), st));
         int per_sm = 0;
-        CRT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_fused_kernel<false>, PANEL_WARPS * 32, 0));
-        P->chol_grid = std::max(1, per_sm * ctx->sm_count);
-        const char* gm = getenv("SFMB200_BA_GRID");
-        P->one_wave = !(gm && strcmp(gm, "legacy") == 0);
-        const char* cm = getenv("SFMB200_BA_CHOL");
-        P->chol_fused = !(cm && strcmp(cm, "steps") == 0) && per_sm > 0;
-        P->chol_lookahead = cm && strcmp(cm, "lookahead") == 0;
-        int per_sm_stream = 0;
-        CRT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_stream, chol_stream_kernel, CS_THREADS, 0));
-        P->chol_grid_stream = std::max(1, per_sm_stream * ctx->sm_count);
-        P->chol_stream = P->chol_fused && per_sm_stream > 0 && !(cm && (strcmp(cm, "fused") == 0 || strcmp(cm, "lookahead") == 0));
-        // back substitution with the next block row staged in shared memory (cp.async) when it fits
-        const char* bm = getenv("SFMB200_BA_BACKSOLVE");
-        const size_t bs = chol_backsolve_smem(P->npad, true);
-        P->backsolve_staged = !(bm && strcmp(bm, "direct") == 0) && bs <= 220 * 1024;
-        if (P->backsolve_staged) {
-            CRT(cudaFuncSetAttribute(chol_backsolve_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs));
-            CRT(cudaFuncSetAttribute(chol_backsolve_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs));
+        CRT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_stream_kernel, CS_THREADS, 0));
+        if (per_sm < 1) {
+            cudaStreamSynchronize(st); ba_release_buffers(P); delete P;
+            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "the dense Cholesky kernel cannot be resident on this device");
         }
-        // back substitution on a cluster of BS_CLUSTER SMs (needs the inverse diagonal tiles the dataflow factorisations leave)
+        P->chol_grid_stream = per_sm * ctx->sm_count;
+        // back substitution on a cluster of BS_CLUSTER SMs while its per-CTA slices fit (n <= 2816, 469 cameras), on one CTA above
         const size_t cs = chol_backsolve_cluster_smem(P->n);
-        const int cthreads = chol_backsolve_cluster_threads(P->n);
-        if (P->chol_fused && !(bm && (strcmp(bm, "direct") == 0 || strcmp(bm, "single") == 0)) && cs <= 200 * 1024 && cthreads <= 512) {
-            CRT(cudaFuncSetAttribute(chol_backsolve_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(BS_CLUSTER); cfg.blockDim = dim3(cthreads); cfg.dynamicSmemBytes = cs;
-            int nclusters = 0;
-            if (cudaOccupancyMaxActiveClusters(&nclusters, chol_backsolve_cluster_kernel, &cfg) == cudaSuccess && nclusters > 0) P->backsolve_cluster = true;
-            else (void)cudaGetLastError();
-        }
+        P->backsolve_cluster = cs <= 200 * 1024 && chol_backsolve_cluster_threads(P->n) <= 512;
+        if (P->backsolve_cluster) CRT(cudaFuncSetAttribute(chol_backsolve_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
     }
     CRT(cudaMemsetAsync(P->counters, 0, 64, st));
     {   // mode: gather (default: ba_pair_kernel + ba_combine_kernel, deterministic) needs the pair-list fill's per-warp camera counters in shared

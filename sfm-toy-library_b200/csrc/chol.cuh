@@ -11,77 +11,22 @@ namespace {
 
 constexpr int NB = 32;                 // Cholesky tile
 
-// Panel step k.  CTA = 4 warps = 128 threads; every CTA factors the 32x32 diagonal tile itself (11 k FMA, cheaper than a
-// cross-CTA dependency) and solves up to four sub-diagonal tiles against it.  A single warp working through the tile is
-// issue-latency bound (measured: ~5 k dependent instructions at IPC 0.09 = 26 us), so the work is restructured:
-//   phase 1  factorisation, lane = row, the 32 columns dealt round-robin to the 4 warps (8 registers each).  Per pivot the
-//            owning warp produces the column (shuffle, rsqrt, scale) and publishes it in shared memory; after ONE barrier
-//            every warp applies it to its 8 columns (8 broadcast-LDS + FMA instead of 31 in one warp).  The register set is
-//            rotated every 4 pivots so that the loop stays rolled with static register indices.
-//   phase 2  each warp solves X L^T = B for its tile, row per lane in registers (rotated like phase 1), L[c][j] as
-//            broadcast LDS.  (An explicit 32x32 inverse + product was measured slower: 15 k + 7 k cycles vs ~5 k.)
-// CTA 0 writes the factor back together with the reciprocal pivots (dinv) the back-substitution uses.  Pivots with
-// global index >= n are forced to 1 with a zero column (augmented rhs row / padding rows).
+// A tile is factored by PANEL_WARPS warps (lane = row, the columns dealt to the warps in groups of four).  A single warp
+// working through the tile is issue-latency bound (measured: ~5 k dependent instructions at IPC 0.09 = 26 us), so every
+// pivot round is split between an owning warp that produces the columns and one barrier after which every warp applies them
+// to its own columns.  Pivots with global index >= n are forced to 1 with a zero column (augmented rhs row / padding rows).
 constexpr int PANEL_WARPS = 4;
 
-// Barrier among the PANEL_WARPS*32 threads that factor a tile.  In a CTA that has more warps (the dataflow kernel's solver
-// warp) this must not be barrier 0.
-template <bool NAMED> __device__ __forceinline__ void chol_factor_barrier() {
-    if (NAMED) asm volatile("bar.sync 1, %0;" :: "n"(PANEL_WARPS * 32) : "memory"); else __syncthreads();
+// Barrier among the PANEL_WARPS*32 threads that factor a tile.  The dataflow kernel's CTA has a fifth warp, so this is not
+// barrier 0.
+__device__ __forceinline__ void chol_factor_barrier() {
+    asm volatile("bar.sync 1, %0;" :: "n"(PANEL_WARPS * 32) : "memory");
 }
 
-// Phase 1 on a 32x32 tile held in registers: col[q] = element (row `lane`, column PANEL_WARPS*q + w).  Leaves the factor
-// (lower triangle, zeros above) in Ls and the reciprocal pivots in invd; ends with a barrier.  gbase = global index of the
-// tile's first pivot.  Returns true if a pivot was not positive.
-// groups_done (optional, shared memory): number of finished 4-column groups, published one pivot after the group's columns
-// are in Ls so that a warp outside the factorisation can stream them out (fence + volatile store / volatile poll + fence).
-template <bool NAMED>
-__device__ __forceinline__ bool chol_tile_factor(double (&col)[NB / PANEL_WARPS], double (*Ls)[NB + 1], double (*colbuf)[NB], double* invd,
-                                                 int lane, int w, int gbase, int n, volatile int* groups_done, int* bad_flag) {
-    bool bad = false;
-#pragma unroll 1
-    for (int jb = 0; jb < NB; jb += PANEL_WARPS) {
-#pragma unroll
-        for (int ow = 0; ow < PANEL_WARPS; ++ow) {                    // pivot j = jb + ow is column col[0] of warp ow
-            const int j = jb + ow, gj = gbase + j;
-            if (w == ow) {
-                const double d = __shfl_sync(0xffffffffu, col[0], j);
-                double ljj, inv;
-                if (gj >= n) { ljj = 1.0; inv = 0.0; }
-                else if (!(d > 0.0) || !isfinite(d)) { bad = true; ljj = 1.0; inv = 1.0; }
-                else { inv = rsqrt(d); ljj = d * inv; }
-                const double lrj = lane == j ? ljj : (lane > j ? col[0] * inv : 0.0);
-                col[0] = lrj;
-                colbuf[j & 1][lane] = lrj;
-                if (lane == j) invd[j] = inv;
-            }
-            chol_factor_barrier<NAMED>();
-            if (ow == 0 && groups_done && jb > 0 && threadIdx.x == 0) { __threadfence_block(); *groups_done = jb / PANEL_WARPS; }
-            const double lrj = colbuf[j & 1][lane];
-#pragma unroll
-            for (int q = 0; q < NB / PANEL_WARPS; ++q) {
-                const int c = jb + PANEL_WARPS * q + w;               // column held in col[q]; >= NB means wrapped (finished)
-                if (c > j && c < NB) col[q] = fma(-lrj, colbuf[j & 1][c], col[q]);
-            }
-        }
-        // the pivot columns of this group are final: store them, rotate the register set by one
-        if (lane >= jb + w) Ls[lane][jb + w] = col[0]; else Ls[lane][jb + w] = 0.0;
-        const double t = col[0];
-#pragma unroll
-        for (int q = 0; q < NB / PANEL_WARPS - 1; ++q) col[q] = col[q + 1];
-        col[NB / PANEL_WARPS - 1] = t;
-    }
-    if (bad) *bad_flag = 1;                        // a pivot is seen by its owning warp only
-    chol_factor_barrier<NAMED>();
-    if (groups_done && threadIdx.x == 0) { __threadfence_block(); *groups_done = NB / PANEL_WARPS; }
-    return *bad_flag != 0;
-}
-
-// Quad-pivot variant of phase 1 (the one the streaming dataflow kernel runs).  History of the chain, per 32-column tile:
-// one barrier per pivot 6.2 us -> pair pivots 4.1 us -> this.  A cycle-stamped trace (tools/chol_microbench.cu built with
-// -DCHOL_FINE_TRACE) showed that the cost of a round is the NUMBER of instructions the owning warp executes between two
-// barriers (a single warp of mostly dependent fp64 code runs at ~5 cycles per instruction), not the depth of the pivot
-// recurrence, so the round is built to be short:
+// Factorisation of a 32x32 tile in quad-pivot rounds.  Measured per 32-column tile: one barrier per pivot 6.2 us, pair
+// pivots 4.1 us.  A cycle-stamped trace (tools/chol_microbench.cu built with -DCHOL_FINE_TRACE) showed that the cost of a
+// round is the NUMBER of instructions the owning warp executes between two barriers (a single warp of mostly dependent fp64
+// code runs at ~5 cycles per instruction), not the depth of the pivot recurrence, so the round is built to be short:
 //   * warp w owns the column QUADS 16q+4w .. 16q+4w+3 (col[q][h], lane = row): one barrier and one shared-memory round trip
 //     serve FOUR pivots;
 //   * the owner fetches the 10 entries of the quad's 4x4 diagonal block with shuffles issued together and every lane
@@ -161,10 +106,10 @@ __device__ __forceinline__ void chol_quad_owner(const double (&a)[4], double (*L
 }
 // col[q][h] = element (row `lane`, column 16q + 4w + h) of the (fully symmetric) tile.  Leaves the factor transposed in LT
 // (LT[j][r] = L(r,j) for r >= j; r < j: round-off, to be masked by the reader) and the reciprocal pivots in invd; ends with a
-// barrier.  stream: warp 0 hands every finished quad to the streaming warp through the quad's named barrier (ids 2..9, 32 + 32
+// barrier.  Warp 0 hands every finished quad to the streaming warp through the quad's named barrier (ids 2..9, 32 + 32
 // threads; warp 0 only arrives) -- a hand-over compute-sanitizer's racecheck can see.
 __device__ __forceinline__ bool chol_tile_factor4(double (&col)[NB / (4 * PANEL_WARPS)][4], double (*LT)[NB], double* invd,
-                                                  int lane, int w, int gbase, int n, bool stream, int* bad_flag) {
+                                                  int lane, int w, int gbase, int n, int* bad_flag) {
     bool bad = false;
     const bool tail = gbase + NB > n;
     if (w == 0) CHOL_FINE(0);
@@ -179,9 +124,9 @@ __device__ __forceinline__ bool chol_tile_factor4(double (&col)[NB / (4 * PANEL_
                 else chol_quad_owner<false>(col[0], LT, invd, lane, j0, gbase, n, bad);
                 CHOL_FINE(2 + (j0 / 4) * 4);
             }
-            chol_factor_barrier<true>();
+            chol_factor_barrier();
             if (w == 0) CHOL_FINE(3 + (j0 / 4) * 4);
-            if (stream && w == 0) { __threadfence_block(); asm volatile("bar.arrive %0, 64;" ::"r"(2 + j0 / 4) : "memory"); }
+            if (w == 0) { __threadfence_block(); asm volatile("bar.arrive %0, 64;" ::"r"(2 + j0 / 4) : "memory"); }
             const double m0 = LT[j0][lane], m1 = LT[j0 + 1][lane], m2 = LT[j0 + 2][lane], m3 = LT[j0 + 3][lane];
 #pragma unroll
             for (int q = 0; q < NB / (4 * PANEL_WARPS); ++q) {
@@ -205,32 +150,14 @@ __device__ __forceinline__ bool chol_tile_factor4(double (&col)[NB / (4 * PANEL_
             for (int h = 0; h < 4; ++h) col[q][h] = col[q + 1][h];
     }
     if (bad) *bad_flag = 1;                        // a pivot is seen by its owning warp only
-    chol_factor_barrier<true>();
+    chol_factor_barrier();
     return *bad_flag != 0;
 }
 
-// Phase 2, pivots jb .. jb+PANEL_WARPS-1, for one warp: X L^T = B for row `lane`, b[] rotated so that b[0] is column jb.
-// L in Ls (rows > pivot of columns jb..jb+3 are read), reciprocal pivots in invd.  Rotates b[] by PANEL_WARPS on return, so
-// that the loop over the groups stays rolled with static register indices; L[c][j] arrives as a broadcast LDS.
-__device__ __forceinline__ void chol_tile_trsm_group(double (&b)[NB], const double (*Ls)[NB + 1], const double* invd, int jb) {
-#pragma unroll
-    for (int u = 0; u < PANEL_WARPS; ++u) {
-        const int j = jb + u;
-        const double xj = b[u] * invd[j];
-        b[u] = xj;
-#pragma unroll
-        for (int p2 = u + 1; p2 < NB; ++p2)
-            if (jb + p2 < NB) b[p2] = fma(-xj, Ls[jb + p2][j], b[p2]);
-    }
-    double t[PANEL_WARPS];
-#pragma unroll
-    for (int u = 0; u < PANEL_WARPS; ++u) t[u] = b[u];
-#pragma unroll
-    for (int p2 = 0; p2 < NB - PANEL_WARPS; ++p2) b[p2] = b[p2 + PANEL_WARPS];
-#pragma unroll
-    for (int u = 0; u < PANEL_WARPS; ++u) b[NB - PANEL_WARPS + u] = t[u];
-}
-// same with the factor stored transposed (LT[j][c] = L(c,j)), as chol_tile_factor4 leaves it
+// One warp solves X L^T = B for row `lane` of B, with the factor stored transposed (LT[j][c] = L(c,j)) as chol_tile_factor4
+// leaves it and the reciprocal pivots in invd.  b[] is rotated by PANEL_WARPS per group of pivots, so that the loop over the
+// groups stays rolled with static register indices (b[0] is always the current pivot's column); L(c,j) arrives as a
+// broadcast LDS.  On return b[] is back in natural order.
 __device__ __forceinline__ void chol_tile_trsm_t(double (&b)[NB], const double (*LT)[NB], const double* invd) {
 #pragma unroll 1
     for (int jb = 0; jb < NB; jb += PANEL_WARPS) {
@@ -252,87 +179,20 @@ __device__ __forceinline__ void chol_tile_trsm_t(double (&b)[NB], const double (
         for (int u = 0; u < PANEL_WARPS; ++u) b[NB - PANEL_WARPS + u] = t[u];
     }
 }
-// all 32 pivots; on return b[] is back in natural order
-__device__ __forceinline__ void chol_tile_trsm(double (&b)[NB], const double (*Ls)[NB + 1], const double* invd) {
-#pragma unroll 1
-    for (int jb = 0; jb < NB; jb += PANEL_WARPS) chol_tile_trsm_group(b, Ls, invd, jb);
-}
-
-// `skip` (all kernels of this file, optional): when it points at a non-zero word the launch is a no-op -- the device-resident
-// LM loop enqueues whole chunks of iterations and the solve may terminate inside one.
-__global__ void __launch_bounds__(PANEL_WARPS * 32) chol_panel_kernel(double* __restrict__ A, int npad, int n, int k, int nbk,
-                                                                      double* __restrict__ dinv, int* __restrict__ fail, const int* __restrict__ skip = nullptr) {
-    if (skip && *skip) return;
-    __shared__ double Ls[NB][NB + 1];          // diagonal tile, then its factor (lower)
-    __shared__ double colbuf[2][NB];
-    __shared__ double invd[NB];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int i = k + 1 + blockIdx.x * PANEL_WARPS + w;
-    const bool has_tile = i < nbk;
-    double b[NB];                               // this warp's sub-diagonal tile, row `lane`
-    if (has_tile) {
-        const double* src = A + (size_t)(i * NB + lane) * npad + k * NB;
-#pragma unroll
-        for (int c = 0; c < NB; c += 2) { const double2 v = *reinterpret_cast<const double2*>(src + c); b[c] = v.x; b[c + 1] = v.y; }
-    }
-    {   // diagonal tile -> shared memory; all 8 loads of a thread are issued before the first store
-        double v[NB * NB / (PANEL_WARPS * 32)];
-#pragma unroll
-        for (int u = 0; u < NB * NB / (PANEL_WARPS * 32); ++u) { const int e = threadIdx.x + u * PANEL_WARPS * 32; v[u] = A[(size_t)(k * NB + (e >> 5)) * npad + k * NB + (e & 31)]; }
-#pragma unroll
-        for (int u = 0; u < NB * NB / (PANEL_WARPS * 32); ++u) { const int e = threadIdx.x + u * PANEL_WARPS * 32; Ls[e >> 5][e & 31] = v[u]; }
-    }
-    __syncthreads();
-    double col[NB / PANEL_WARPS];
-#pragma unroll
-    for (int q = 0; q < NB / PANEL_WARPS; ++q) col[q] = Ls[lane][PANEL_WARPS * q + w];
-    __shared__ int bad_flag;
-    if (threadIdx.x == 0) bad_flag = 0;
-    const bool bad = chol_tile_factor<false>(col, Ls, colbuf, invd, lane, w, k * NB, n, nullptr, &bad_flag);
-    if (bad && threadIdx.x == 0 && blockIdx.x == 0) atomicAdd(fail, 1);
-    if (blockIdx.x == 0) {
-        for (int e = threadIdx.x; e < NB * NB; e += PANEL_WARPS * 32) { const int r = e >> 5, c = e & 31; if (c <= r) A[(size_t)(k * NB + r) * npad + k * NB + c] = Ls[r][c]; }
-        if (threadIdx.x < NB) dinv[k * NB + threadIdx.x] = invd[threadIdx.x];
-    }
-    if (!has_tile) return;
-    chol_tile_trsm(b, Ls, invd);
-    double* dst = A + (size_t)(i * NB + lane) * npad + k * NB;
-#pragma unroll
-    for (int c = 0; c < NB; c += 2) *reinterpret_cast<double2*>(dst + c) = make_double2(b[c], b[c + 1]);
-}
-
-// Trailing update step k: tile (i, j), k < j <= i:  A[i][j] -= A[i][k] A[j][k]^T.  blockDim = (32, 32), grid = T(T+1)/2.
-__global__ void __launch_bounds__(1024) chol_update_kernel(double* __restrict__ A, int npad, int k, int nbk, const int* __restrict__ skip = nullptr) {
-    if (skip && *skip) return;
-    __shared__ double P[NB][NB + 1], Q[NB][NB + 1];
-    // decode blockIdx.x -> (i, j) over the lower triangle of the trailing (T x T) tile matrix
-    int t = blockIdx.x, ii = 0;
-    while (t > ii) { t -= ii + 1; ++ii; }
-    const int i = k + 1 + ii, j = k + 1 + t;
-    (void)nbk;
-    const int r = threadIdx.y, c = threadIdx.x;
-    P[r][c] = A[(size_t)(i * NB + r) * npad + k * NB + c];
-    Q[r][c] = A[(size_t)(j * NB + r) * npad + k * NB + c];
-    __syncthreads();
-    double s = 0;
-#pragma unroll 8
-    for (int m = 0; m < NB; ++m) s += P[r][m] * Q[c][m];
-    if (i != j || c <= r) A[(size_t)(i * NB + r) * npad + j * NB + c] -= s;
-}
 
 // ---------------------------------------------------------------------------------------------------------------
-// K4 (default): the whole factorisation as ONE persistent dataflow kernel (left-looking tile Cholesky).
-// The step-wise version above pays a kernel boundary + a cold L2 round trip twice per 32 columns (19 panel + 18 update
-// launches at 100 cameras, ~390 us) although the arithmetic is 72 MFLOP.  Here every lower-triangle tile (i, c) has one owner
-// CTA that keeps it in registers (phase-1 layout) for its whole life:
+// K4: the whole factorisation as ONE persistent dataflow kernel (left-looking tile Cholesky).  A panel kernel and an update
+// kernel per 32 columns would pay a kernel boundary and a cold L2 round trip twice per 32 columns (19 + 18 launches at 100
+// cameras, ~390 us measured) although the arithmetic is 72 MFLOP.  Here every lower-triangle tile (i, c) has one owner CTA
+// that keeps it in registers for its whole life:
 //     for k < c:  wait ready(i,k), ready(c,k);  tile -= L(i,k) L(c,k)^T            (operands through shared memory)
-//     i == c:     factor the tile (chol_tile_factor), store L(c,c) + reciprocal pivots, publish ready(c,c)
-//     i >  c:     wait ready(c,c);  one warp solves X L(c,c)^T = tile (chol_tile_trsm), stores L(i,c), publishes ready(i,c)
-// LOOKAHEAD: the critical path runs down the diagonal, factor(c) -> solve(c+1,c) -> update -> factor(c+1); with separate
-// owners that is two global-memory hand-overs per 32 columns.  So the first sub-diagonal tile (c+1,c) and the diagonal tile
-// (c+1,c+1) share one owner: it carries both tiles through the updates, solves (c+1,c), applies it to the diagonal tile
+//     i == c:     factor the tile (chol_tile_factor4), store L(c,c) + reciprocal pivots, publish it
+//     i >  c:     wait for L(c,c);  solve X L(c,c)^T = tile, store L(i,c), publish ready(i,c)
+// The critical path runs down the diagonal, factor(c) -> solve(c+1,c) -> update -> factor(c+1); with separate owners that is
+// two global-memory hand-overs per 32 columns.  So the first sub-diagonal tile (c+1,c) and the diagonal tile (c+1,c+1) share
+// one owner (the "merged" task): it carries both tiles through the updates, solves (c+1,c), applies it to the diagonal tile
 // straight from shared memory and factors -- one hand-over per 32 columns.
-// Publishing = all stores, barrier, __threadfence + a store of the solve's epoch number into ready[] (no reset between
+// Publishing a tile = all stores, barrier, __threadfence + a store of the solve's epoch number into ready[] (no reset between
 // solves); consuming = every thread polls (relaxed), fences, then reads the tile with ld.global.cg (L1 may hold the
 // pre-factor values of a tile another CTA of this SM owned).
 // Deadlock freedom: tasks are numbered column-major (the merged task sits in column c) and dealt round-robin, each CTA works
@@ -371,162 +231,22 @@ __device__ __forceinline__ void tile_publish(unsigned* flag, unsigned epoch) {
     __threadfence();
     st_relaxed_gpu_u32(flag, epoch);
 }
-// 32x32 tile at A[row0.., col0..] -> shared memory, bypassing L1; the 4 loads of a thread are issued before the first store
-__device__ __forceinline__ void tile_to_smem(double (*T)[NB + 1], const double* __restrict__ A, int npad, int row0, int col0) {
-    double2 v[NB * NB / (2 * PANEL_WARPS * 32)];
-#pragma unroll
-    for (int u = 0; u < NB * NB / (2 * PANEL_WARPS * 32); ++u) {
-        const int e = threadIdx.x + u * PANEL_WARPS * 32, r = e >> 4, c = (e & 15) * 2;
-        v[u] = __ldcg(reinterpret_cast<const double2*>(A + (size_t)(row0 + r) * npad + col0 + c));
-    }
-#pragma unroll
-    for (int u = 0; u < NB * NB / (2 * PANEL_WARPS * 32); ++u) {
-        const int e = threadIdx.x + u * PANEL_WARPS * 32, r = e >> 4, c = (e & 15) * 2;
-        T[r][c] = v[u].x; T[r][c + 1] = v[u].y;
-    }
-}
-// shared memory tile -> A[row0.., col0..], coalesced 16-byte stores
-__device__ __forceinline__ void smem_to_tile(double* __restrict__ A, int npad, int row0, int col0, const double (*T)[NB + 1]) {
-#pragma unroll
-    for (int u = 0; u < NB * NB / (2 * PANEL_WARPS * 32); ++u) {
-        const int e = threadIdx.x + u * PANEL_WARPS * 32, r = e >> 4, c = (e & 15) * 2;
-        *reinterpret_cast<double2*>(A + (size_t)(row0 + r) * npad + col0 + c) = make_double2(T[r][c], T[r][c + 1]);
-    }
-}
-// acc (phase-1 layout) -= P Q^T
-__device__ __forceinline__ void tile_rank32_update(double (&acc)[NB / PANEL_WARPS], const double (*P)[NB + 1], const double (*Q)[NB + 1], int lane, int w) {
-#pragma unroll 4
-    for (int m = 0; m < NB; ++m) {
-        const double pv = P[lane][m];
-#pragma unroll
-        for (int q = 0; q < NB / PANEL_WARPS; ++q) acc[q] = fma(-pv, Q[PANEL_WARPS * q + w][m], acc[q]);
-    }
-}
+// number of tasks of the dataflow kernel for nbk tile rows: column 0 holds nbk tiles, every later column c one tile fewer
+// than its length because its diagonal tile rides with the merged task of column c-1
+__host__ __device__ inline int chol_stream_tasks(int nbk) { return nbk + (nbk - 1) * (nbk - 2) / 2; }
 
-// number of tasks of the dataflow kernel for nbk tile rows
-__host__ __device__ inline int chol_fused_tasks(int nbk, bool lookahead) {
-    return lookahead ? nbk + (nbk - 1) * (nbk - 2) / 2 : nbk * (nbk + 1) / 2;
-}
-
-// trace (optional, tools/chol_microbench.cu): 8 x u64 %globaltimer stamps per task:
-//   0 start, 1 updates done, 2 diagonal tile seen, 3 solve done, 4 (i,c) published, 5 factor done, 6 (i,i) published
-template <bool LOOKAHEAD>
-__global__ void __launch_bounds__(PANEL_WARPS * 32) chol_fused_kernel(double* __restrict__ A, int npad, int n, int nbk, int ntasks,
-                                                                      double* __restrict__ dinv, int* __restrict__ fail,
-                                                                      unsigned* __restrict__ ready, unsigned epoch,
-                                                                      double* __restrict__ Linv, unsigned long long* __restrict__ trace,
-                                                                      const int* __restrict__ skip = nullptr, const unsigned* __restrict__ epoch_dev = nullptr) {
-    if (skip && *skip) return;
-    if (epoch_dev) epoch = *epoch_dev;       // CUDA-graph replays: the solve number lives on the device (kernel arguments are frozen)
-    __shared__ double Ps[NB][NB + 1], Qs[NB][NB + 1];
-    __shared__ double colbuf[2][NB];
-    __shared__ double invd[NB];
-    __shared__ int bad_flag;
-    if (threadIdx.x == 0) bad_flag = 0;
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#define CHOL_TRACE(slot) do { if (trace && threadIdx.x == 0) trace[(size_t)t * 8 + (slot)] = chol_globaltimer(); } while (0)
-    for (int t = blockIdx.x; t < ntasks; t += gridDim.x) {
-        int i, c; bool merged = false;
-        if (!LOOKAHEAD) {
-            int rem = t; c = 0;
-            while (rem >= nbk - c) { rem -= nbk - c; ++c; }        // column-major over the lower triangle
-            i = c + rem;
-        } else if (t == 0) { i = c = 0; }
-        else {
-            int rem = t - 1, cnt = nbk - 1; c = 0;
-            while (rem >= cnt) { rem -= cnt; ++c; cnt = nbk - 1 - c; }   // column c: tiles (c+1..nbk-1, c); (c+1,c) carries (c+1,c+1)
-            i = c + 1 + rem; merged = rem == 0;
-        }
-        CHOL_TRACE(0);
-        double col[NB / PANEL_WARPS], col2[NB / PANEL_WARPS];
-#pragma unroll
-        for (int q = 0; q < NB / PANEL_WARPS; ++q) {
-            col[q] = __ldcg(A + (size_t)(i * NB + lane) * npad + c * NB + PANEL_WARPS * q + w);
-            col2[q] = merged ? __ldcg(A + (size_t)(i * NB + lane) * npad + i * NB + PANEL_WARPS * q + w) : 0.0;
-        }
-        for (int k = 0; k < c; ++k) {
-            bool ok = tile_wait(ready + i * nbk + k, epoch);
-            if (i != c) ok = tile_wait(ready + c * nbk + k, epoch) && ok;
-            tile_to_smem(Ps, A, npad, i * NB, k * NB);
-            if (i != c) tile_to_smem(Qs, A, npad, c * NB, k * NB);
-            if (!__syncthreads_and(ok)) { if (threadIdx.x == 0) atomicAdd(fail, 1000); return; }
-            tile_rank32_update(col, Ps, (i == c) ? Ps : Qs, lane, w);
-            if (merged) tile_rank32_update(col2, Ps, Ps, lane, w);
-            __syncthreads();
-        }
-        CHOL_TRACE(1);
-        if (i != c) {
-            const bool ok = tile_wait(ready + c * nbk + c, epoch);
-            CHOL_TRACE(2);
-            tile_to_smem(Qs, A, npad, c * NB, c * NB);              // only its lower triangle is read
-            if (threadIdx.x < NB) invd[threadIdx.x] = __ldcg(dinv + c * NB + threadIdx.x);
-#pragma unroll
-            for (int q = 0; q < NB / PANEL_WARPS; ++q) Ps[lane][PANEL_WARPS * q + w] = col[q];
-            if (!__syncthreads_and(ok)) { if (threadIdx.x == 0) atomicAdd(fail, 1000); return; }
-            if (w == 0) {
-                double b[NB];
-#pragma unroll
-                for (int q = 0; q < NB; ++q) b[q] = Ps[lane][q];
-                chol_tile_trsm(b, Qs, invd);
-                if (!merged) {
-                    double* dst = A + (size_t)(i * NB + lane) * npad + c * NB;
-#pragma unroll
-                    for (int q = 0; q < NB; q += 2) *reinterpret_cast<double2*>(dst + q) = make_double2(b[q], b[q + 1]);
-                } else {
-#pragma unroll
-                    for (int q = 0; q < NB; ++q) Ps[lane][q] = b[q];
-                }
-            }
-            __syncthreads();                                        // non-merged: stores issued; merged: X in Ps
-            CHOL_TRACE(3);
-            if (merged) {
-                smem_to_tile(A, npad, i * NB, c * NB, Ps);
-                tile_rank32_update(col2, Ps, Ps, lane, w);
-                __syncthreads();                                    // stores of X issued by every thread; Ps, Qs free
-            }
-            if (threadIdx.x == 0) tile_publish(ready + i * nbk + c, epoch);
-            CHOL_TRACE(4);
-        }
-        if (i == c || merged) {
-            if (merged) {               // one register array into the factorisation (a runtime choice of array costs 2x)
-#pragma unroll
-                for (int q = 0; q < NB / PANEL_WARPS; ++q) col[q] = col2[q];
-            }
-            const bool bad = chol_tile_factor<false>(col, Qs, colbuf, invd, lane, w, i * NB, n, nullptr, &bad_flag);
-            if (bad && threadIdx.x == 0) atomicAdd(fail, 1);
-            CHOL_TRACE(5);
-            for (int e = threadIdx.x; e < NB * NB; e += PANEL_WARPS * 32) { const int r = e >> 5, q = e & 31; if (q <= r) A[(size_t)(i * NB + r) * npad + i * NB + q] = Qs[r][q]; }
-            if (threadIdx.x < NB) dinv[i * NB + threadIdx.x] = invd[threadIdx.x];
-            __syncthreads();
-            if (threadIdx.x == 0) tile_publish(ready + i * nbk + i, epoch);
-            CHOL_TRACE(6);
-            if (Linv && w == 0) {       // off the critical path: L(i,i)^-1 (row-major) for the back substitution.  X L^T = I, X = L^-T
-                double b[NB];
-#pragma unroll
-                for (int q = 0; q < NB; ++q) b[q] = lane == q ? 1.0 : 0.0;
-                chol_tile_trsm(b, Qs, invd);
-#pragma unroll
-                for (int q = 0; q < NB; ++q) Linv[((size_t)i * NB + q) * NB + lane] = b[q];      // Linv[q][lane] = X[lane][q]
-            }
-        }
-        __syncthreads();                                            // shared memory is reused by the next task
-    }
-#undef CHOL_TRACE
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// K4, streaming dataflow kernel (default).  Same task graph as chol_fused_kernel<LOOKAHEAD = true>, restructured around what
-// its timeline showed (tools/chol_microbench.cu): per 32 columns the chain spent 5.4 us in the factorisation, 4.6 us in the
-// solve that FOLLOWED it, 1.5 us in the SIMT rank-32 update and only 0.75 us in the hand-over.  So:
+// The shape of the kernel follows a timeline of the chain (tools/chol_microbench.cu).  With four warps that factor, then
+// solve, then update with SIMT FMAs, each 32 columns spent 5.4 us in the factorisation, 4.6 us in the solve that FOLLOWED
+// it, 1.5 us in the rank-32 update and only 0.75 us in the hand-over.  So:
 //   * the factor of a diagonal tile is streamed out in groups of 4 columns while it is being computed: a fifth warp of the
-//     owner CTA copies the finished columns from shared memory to A, fences and bumps progress[c]; every solve of that tile
+//     owner CTA copies the finished columns from shared memory to A and to the LL lines below; every solve of that tile
 //     column consumes the groups as they arrive and finishes a fraction of a microsecond after the factorisation instead
 //     of 4.6 us later (the solve keeps pace: 134 ns per pivot against 190 ns);
 //   * the rank-32 updates run on the FP64 tensor pipe (mma.sync.m8n8k4.f64, accumulators in fragment layout for the whole
 //     life of the tile, operands from shared memory with a conflict-free 36-double row stride): 40 LDS + 32 DMMA per warp
 //     instead of 288 LDS + 256 DFMA;
-//   * the fifth warp is also the solver warp, and afterwards produces L(c,c)^-1 for the back substitution.
-// progress[c] = 16 * epoch + number of published groups (monotonic over solves, no reset); ready[] as before for tiles.
+//   * the fifth warp also hands the streamed groups to the solve of its own CTA, and after a factorisation produces
+//     L(c,c)^-1 for the back substitution.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int CS_THREADS = PANEL_WARPS * 32 + 32;
 constexpr int TS = NB + 4;              // row stride of the DMMA operand tiles
@@ -588,6 +308,10 @@ __device__ __forceinline__ bool ll_try(const uint4* line, unsigned tag, double& 
     return b == tag && d == tag;
 }
 
+// `skip` (every kernel of this file, optional): when it points at a non-zero word the launch is a no-op -- the device-resident
+// LM loop enqueues whole chunks of iterations and the solve may terminate inside one.
+// trace (optional, tools/chol_microbench.cu): 8 x u64 %globaltimer stamps per task: 0 start, 1 updates done, 2 first group of
+// L(c,c) seen, 3 solve done, 4 (i,c) published, 5 factor done, 6 factor streamed out, 7 factor start
 __global__ void __launch_bounds__(CS_THREADS) chol_stream_kernel(double* __restrict__ A, int npad, int n, int nbk, int ntasks,
                                                                  double* __restrict__ dinv, int* __restrict__ fail,
                                                                  unsigned* __restrict__ ready, uint4* __restrict__ ll, unsigned epoch,
@@ -748,7 +472,7 @@ __global__ void __launch_bounds__(CS_THREADS) chol_stream_kernel(double* __restr
                     const double v0 = merged ? c2[cb][0] : c1[cb][0], v1 = merged ? c2[cb][1] : c1[cb][1];
                     *reinterpret_cast<double2*>(&Pt[8 * w + fr][8 * cb + 2 * fc]) = make_double2(v0, v1);
                 }
-                chol_factor_barrier<true>();
+                chol_factor_barrier();
                 CHOL_TRACE(7);
                 double col[NB / (4 * PANEL_WARPS)][4];
 #pragma unroll
@@ -757,7 +481,7 @@ __global__ void __launch_bounds__(CS_THREADS) chol_stream_kernel(double* __restr
                     const double2 v2 = *reinterpret_cast<const double2*>(&Pt[lane][4 * PANEL_WARPS * q + 4 * w + 2]);
                     col[q][0] = v.x; col[q][1] = v.y; col[q][2] = v2.x; col[q][3] = v2.y;
                 }
-                const bool bad = chol_tile_factor4(col, LT, invd, lane, w, i * NB, n, true, &bad_flag);
+                const bool bad = chol_tile_factor4(col, LT, invd, lane, w, i * NB, n, &bad_flag);
                 if (bad && threadIdx.x == 0) atomicAdd(fail, 1);
                 CHOL_TRACE(5);
             } else {
@@ -798,93 +522,43 @@ __global__ void __launch_bounds__(CS_THREADS) chol_stream_kernel(double* __restr
 #undef CHOL_TRACE_W4
 }
 
-// Back substitution L^T x = y with y = row n of the factored matrix.  Single CTA of 640 threads (warp 0 + 608 workers).
-// Per 32-block (descending) warp 0 produces the block's unknowns, then worker c subtracts  sum_m L[kb*32+m][c] x_m  from
-// y[c] for the columns to the left.  The chain of 19 blocks is pure latency, so
-//   STAGED   every thread copies ITS column of the next block row (warp 0: its column of the next diagonal tile) into shared
-//            memory with cp.async one block ahead and picks it up with 32 LDS -- the L2 round trip leaves the chain; a thread
-//            only ever touches its own slots, so a single buffer needs no extra barrier;
-//   USE_INV  warp 0 multiplies by L(kb,kb)^-1 (written by the dataflow factorisation, off its critical path) -- one
-//            32-term dot product per lane instead of 32 dependent shuffle/FMA steps.
+// Back substitution L^T x = y with y = row n of the factored matrix, on one CTA of 640 threads (warp 0 + 608 workers); the
+// kernel for systems too large for the cluster kernel below.  Per 32-block (descending) warp 0 produces the block's unknowns
+// by multiplying with L(kb,kb)^-1 (written by the dataflow factorisation, off its critical path) -- one 32-term dot product
+// per lane instead of 32 dependent shuffle/FMA steps -- then worker c subtracts  sum_m L[kb*32+m][c] x_m  from y[c] for the
+// columns to the left.
 __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" :: "r"(d), "l"(gsrc) : "memory");
 }
-__host__ __device__ inline size_t chol_backsolve_smem(int npad, bool staged) {
-    return sizeof(double) * ((size_t)npad + (staged ? (size_t)NB * NB + (size_t)NB * npad : 0));
-}
+__host__ __device__ inline size_t chol_backsolve_smem(int npad) { return sizeof(double) * (size_t)npad; }
 
-template <bool STAGED, bool USE_INV>
-__global__ void __launch_bounds__(640) chol_backsolve_kernel(const double* __restrict__ A, const double* __restrict__ dinv, const double* __restrict__ Linv,
+__global__ void __launch_bounds__(640) chol_backsolve_kernel(const double* __restrict__ A, const double* __restrict__ Linv,
                                                              int npad, int n, double* __restrict__ x, const int* __restrict__ skip = nullptr) {
     if (skip && *skip) return;
     extern __shared__ double sm[];
     double* y = sm;                               // [npad]
-    double* dstage = sm + npad;                   // [NB][NB]    warp 0's next tile
-    double* stage = dstage + NB * NB;             // [NB][npad]  next block row, column c owned by worker c
     const int tid = threadIdx.x, lane = tid & 31, nworkers = blockDim.x - 32, c0 = tid - 32;
     const bool solver = tid < 32;
     const int kb_first = (n - 1) / NB;
-    // warp 0's 32 values of block kb: column `lane` of L(kb,kb)^-1 (row-major) or of the diagonal tile itself
-    auto solver_src = [&](int kb, int m) -> const double* {
-        return USE_INV ? Linv + ((size_t)kb * NB + m) * NB + lane : A + (size_t)(kb * NB + m) * npad + kb * NB + lane;
-    };
-    auto issue = [&](int kb) {
-        if (kb >= 0) {
-            if (solver) {
-#pragma unroll
-                for (int m = 0; m < NB; ++m) cp_async8(dstage + m * NB + lane, solver_src(kb, m));
-            } else if (c0 < kb * NB) {
-#pragma unroll
-                for (int m = 0; m < NB; ++m) cp_async8(stage + (size_t)m * npad + c0, A + (size_t)(kb * NB + m) * npad + c0);
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    if (STAGED) issue(kb_first);
     for (int i = tid; i < npad; i += blockDim.x) y[i] = i < n ? A[(size_t)n * npad + i] : 0.0;
     __syncthreads();
     for (int kb = kb_first; kb >= 0; --kb) {
         const int ncols = kb * NB;                // columns to the left of the diagonal tile
         const bool has = !solver && c0 < ncols;
-        // one register array, two roles: warp 0 -> its column of the tile; worker c0 -> its column of the block row
+        // one register array, two roles: warp 0 -> column `lane` of L(kb,kb)^-1 (row-major); worker c0 -> its column of the block row
         double reg[NB];
-        if (STAGED) {
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
-            if (solver) {
 #pragma unroll
-                for (int m = 0; m < NB; ++m) reg[m] = dstage[m * NB + lane];
-            } else if (has) {
+        for (int m = 0; m < NB; ++m) reg[m] = solver ? Linv[((size_t)kb * NB + m) * NB + lane] : A[(size_t)(kb * NB + m) * npad + (has ? c0 : 0)];
+        if (solver) {                             // x_r = sum_c Linv[c][r] y_c   (Linv lower triangular: exact zeros for c < r)
+            double s0 = 0, s1 = 0, s2 = 0, s3 = 0;
 #pragma unroll
-                for (int m = 0; m < NB; ++m) reg[m] = stage[(size_t)m * npad + c0];
+            for (int c = 0; c < NB; c += 4) {
+                s0 = fma(reg[c], y[kb * NB + c], s0); s1 = fma(reg[c + 1], y[kb * NB + c + 1], s1);
+                s2 = fma(reg[c + 2], y[kb * NB + c + 2], s2); s3 = fma(reg[c + 3], y[kb * NB + c + 3], s3);
             }
-            issue(kb - 1);
-        } else {
-#pragma unroll
-            for (int m = 0; m < NB; ++m) reg[m] = solver ? *solver_src(kb, m) : A[(size_t)(kb * NB + m) * npad + (has ? c0 : 0)];
-        }
-        if (solver) {
-            if (USE_INV) {                        // x_r = sum_c Linv[c][r] y_c   (Linv lower triangular: exact zeros for c < r)
-                double s0 = 0, s1 = 0, s2 = 0, s3 = 0;
-#pragma unroll
-                for (int c = 0; c < NB; c += 4) {
-                    s0 = fma(reg[c], y[kb * NB + c], s0); s1 = fma(reg[c + 1], y[kb * NB + c + 1], s1);
-                    s2 = fma(reg[c + 2], y[kb * NB + c + 2], s2); s3 = fma(reg[c + 3], y[kb * NB + c + 3], s3);
-                }
-                __syncwarp();
-                y[kb * NB + lane] = (s0 + s1) + (s2 + s3);
-            } else {
-                double yc = y[kb * NB + lane];
-                const double di = dinv[kb * NB + lane];          // reciprocal pivot (0 for padding rows)
-#pragma unroll
-                for (int jj = 0; jj < NB; ++jj) {
-                    const int j = NB - 1 - jj;
-                    double xj = (lane == j) ? yc * di : 0.0;
-                    xj = __shfl_sync(0xffffffffu, xj, j);
-                    if (lane == j) yc = xj; else if (lane < j) yc = fma(-reg[j], xj, yc);
-                }
-                y[kb * NB + lane] = yc;
-            }
+            __syncwarp();
+            y[kb * NB + lane] = (s0 + s1) + (s2 + s3);
         }
         __syncthreads();
         if (has) {
@@ -909,11 +583,11 @@ __global__ void __launch_bounds__(640) chol_backsolve_kernel(const double* __res
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
-// Back substitution on a thread-block CLUSTER (default when L(kb,kb)^-1 tiles exist).  The single-CTA kernel above is bound by
-// ONE SM's shared-memory bandwidth: every block row (32 x n doubles) is written to and read from shared memory once per step,
-// ~2 us per 32 unknowns.  Here BS_CLUSTER CTAs on BS_CLUSTER SMs share the columns -- CTA r owns the 32-column blocks b with
-// b mod BS_CLUSTER = r: their part of y, their slice of every block row (staged with cp.async one step ahead, as above), and the
-// solve of those blocks.  Per step the CTA that owns block kb turns y_kb into x_kb with the inverse tile (one 32-term dot product
+// Back substitution on a thread-block CLUSTER, for every system whose slices fit (chol_backsolve_cluster_smem / _threads).  One
+// CTA that stages every block row (32 x n doubles) in its shared memory is bound by that SM's shared-memory bandwidth, ~2 us
+// per 32 unknowns.  Here BS_CLUSTER CTAs on BS_CLUSTER SMs share the columns -- CTA r owns the 32-column blocks b with
+// b mod BS_CLUSTER = r: their part of y, their slice of every block row (staged with cp.async, each thread into its own
+// slots, so the L2 round trip leaves the chain), and the solve of those blocks.  Per step the CTA that owns block kb turns y_kb into x_kb with the inverse tile (one 32-term dot product
 // per lane) and pushes the 32 values into every CTA's shared memory with st.async, which signals that CTA's mbarrier for the step
 // (complete_tx; armed locally with expect_tx = 256 bytes); every CTA waits on its own mbarrier and subtracts the block row's
 // contribution from its columns (slices staged TWO steps ahead: the L2 latency of a block row exceeds a step).  No cluster-wide barrier inside the loop: one DSMEM hop (~215 cycles) per step.

@@ -1,22 +1,26 @@
-"""Scheduling logic of the dataflow Cholesky kernels (csrc/chol.cuh), modelled on the CPU: the task decode enumerates every
-lower-triangle tile exactly once, every dependency of a task belongs to an EARLIER task, and a grid of G persistent CTAs that
-deal the tasks round-robin and work through them in ascending order always finishes (no spin-wait can deadlock), for any
-number of tile rows and any grid size -- including far more tasks than CTAs, which the GPU tests only touch at one size."""
+"""Scheduling logic of the dataflow Cholesky kernel (chol_stream_kernel, csrc/chol.cuh), modelled on the CPU: the task decode
+enumerates every lower-triangle tile exactly once, every dependency of a task belongs to an EARLIER task, and a grid of G
+persistent CTAs that deal the tasks round-robin and work through them in ascending order always finishes (no spin-wait can
+deadlock), for any number of tile rows and any grid size -- including far more tasks than CTAs, which the GPU tests only touch
+at one size.
+lookahead=True is the kernel's numbering: the diagonal tile (c+1, c+1) rides with the task of (c+1, c).  lookahead=False is the
+numbering it is derived from, one task per tile in column-major order; the deadlock argument in chol.cuh (column-major
+numbering, round-robin dealing, ascending order per CTA) is checked for both, so that it is seen not to rest on the merge."""
 import pytest
 
 
-def n_tasks(nbk, lookahead):                     # chol_fused_tasks
+def n_tasks(nbk, lookahead):                     # lookahead: chol_stream_tasks
     return nbk + (nbk - 1) * (nbk - 2) // 2 if lookahead else nbk * (nbk + 1) // 2
 
 
 def decode(t, nbk, lookahead):
     """-> (i, c, merged): the tile (i, c) of task t; merged tasks also factor the diagonal tile (i, i)."""
-    if not lookahead:                            # chol_fused_kernel<false>: column-major over the lower triangle
+    if not lookahead:                            # one task per tile, column-major over the lower triangle
         rem, c = t, 0
         while rem >= nbk - c:
             rem -= nbk - c; c += 1
         return c + rem, c, False
-    if t == 0:                                   # chol_fused_kernel<true> / chol_stream_kernel
+    if t == 0:                                   # chol_stream_kernel
         return 0, 0, False
     rem, cnt, c = t - 1, nbk - 1, 0
     while rem >= cnt:

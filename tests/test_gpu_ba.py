@@ -177,22 +177,22 @@ def test_red_and_gather_schur_modes_agree(ctx, oracle, monkeypatch):
     np.testing.assert_allclose(out["gather"][2][1], out["red"][2][1], rtol=0, atol=1e-8)
 
 
-@pytest.mark.parametrize("n_cams,n_pts", [(5, 400), (40, 3000), (100, 6000), (180, 5000)])
-def test_dataflow_and_stepwise_cholesky_agree(ctx, monkeypatch, n_cams, n_pts):
-    """The single-kernel dataflow tile Cholesky (streaming = default, plain, lookahead) against the panel/update kernel
-    sequence: same LM trajectory.
-    1 / 8 / 19 / 34 tile rows; the last case has more tiles (595) than co-resident CTAs, so CTAs own several tiles."""
-    p = synth.make_ba_problem(n_cams=n_cams, n_pts=n_pts, obs_per_pt=min(6, n_cams), seed=21)
-    out = {}
-    for mode in ("stream", "fused", "lookahead", "steps"):
-        monkeypatch.setenv("SFMB200_BA_CHOL", mode)
-        monkeypatch.setenv("SFMB200_BA_BACKSOLVE", "direct" if mode == "lookahead" else "staged")
-        prob = ctx.ba_problem(*_args(p))
-        o = capi.ba_default_options(); o.max_num_iterations = 8
-        out[mode] = (prob.run(o), prob.download())
-        prob.close()
-    for m in ("stream", "fused", "lookahead"):
-        _same_trajectory(out[m], out["steps"])
+@pytest.mark.parametrize("n_cams,n_pts,k,iters", [(5, 400, 5, 8), (40, 3000, 6, 8), (100, 6000, 6, 8), (180, 5000, 6, 8), (480, 3000, 4, 3)])
+def test_dense_solve_matches_oracle_trajectory(ctx, oracle, n_cams, n_pts, k, iters):
+    """The dense solve (dataflow tile Cholesky + back substitution) inside whole LM iterations, against the oracle's trajectory.
+    1 / 8 / 19 / 34 tile rows; 180 cameras have more tiles (595) than co-resident CTAs, so CTAs own several tiles.  Up to
+    469 cameras (n = 6 cams + 1 <= 2816) the back substitution runs on a CTA cluster; 480 cameras (n = 2881) are past the
+    cluster kernel's shared-memory limit and take the single-CTA back substitution."""
+    import os
+    p = synth.make_ba_problem(n_cams=n_cams, n_pts=n_pts, obs_per_pt=k, seed=21)
+    opts = dict(max_num_iterations=iters, max_solver_time_in_seconds=0.0)
+    prob = ctx.ba_problem(*_args(p))
+    a = (prob.run(capi.ba_default_options(**opts)), prob.download())
+    prob.close()
+    nthr = max(1, min(32, (os.cpu_count() or 1)))
+    co, po, fo, so = oracle.ba_solve(*_args(p), oracle.ba_default_options(jacobian_mode=1, num_threads=nthr, **opts))
+    assert (a[0]["num_successful_steps"], a[0]["num_unsuccessful_steps"]) == (so["num_successful_steps"], so["num_unsuccessful_steps"]), (a[0], so)
+    _same_trajectory(a, (so, (co, po, fo)))
 
 
 def _same_trajectory(a, b):

@@ -1,6 +1,6 @@
-// tools/chol_microbench.cu -- K4 in isolation: the step-wise panel/update sequence against the dataflow kernel (with and
-// without lookahead) on an SPD matrix of the reduced-camera-system size, checked against a host factorisation, plus the
-// critical-path timeline of the dataflow kernel from its %globaltimer trace.
+// tools/chol_microbench.cu -- K4 in isolation: the streaming dataflow Cholesky kernel on an SPD matrix of the
+// reduced-camera-system size, checked against a host factorisation, with the critical-path timeline from its %globaltimer
+// trace; then the cluster and the single-CTA back-solves on its factor, checked against a host solve.
 // Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -o tools/_build/chol_microbench tools/chol_microbench.cu
 // Usage: chol_microbench [cams=100] [reps=20]
 #include <algorithm>
@@ -12,10 +12,9 @@
 
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e)); return 1; } } while (0)
 
-template <bool LA>
+// task t of chol_stream_kernel -> tile (i, c); merged tasks also factor (i, i)
 static void decode(int t, int nbk, int& i, int& c, bool& merged) {
     merged = false;
-    if (!LA) { int rem = t; c = 0; while (rem >= nbk - c) { rem -= nbk - c; ++c; } i = c + rem; return; }
     if (t == 0) { i = c = 0; return; }
     int rem = t - 1, cnt = nbk - 1; c = 0;
     while (rem >= cnt) { rem -= cnt; ++c; cnt = nbk - 1 - c; }
@@ -53,12 +52,10 @@ int main(int argc, char** argv) {
     unsigned epoch = 0;
     std::vector<double> out((size_t)npad * npad);
     std::vector<unsigned long long> tr((size_t)8 * nbk * nbk);
-    for (int variant = 0; variant < 4; ++variant) {
-        int per_sm = 0, grid = 0, ntasks = 0;
-        if (variant == 1) { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_fused_kernel<false>, PANEL_WARPS * 32, 0)); ntasks = chol_fused_tasks(nbk, false); }
-        if (variant == 2) { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_fused_kernel<true>, PANEL_WARPS * 32, 0)); ntasks = chol_fused_tasks(nbk, true); }
-        if (variant == 3) { CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_stream_kernel, CS_THREADS, 0)); ntasks = chol_fused_tasks(nbk, true); }
-        grid = std::min(ntasks, per_sm * prop.multiProcessorCount);
+    {
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_stream_kernel, CS_THREADS, 0));
+        const int ntasks = chol_stream_tasks(nbk), grid = std::min(ntasks, per_sm * prop.multiProcessorCount);
         float total = 0, best = 1e30f;
         for (int rep = 0; rep < reps + 2; ++rep) {
             const bool traced = rep == reps + 1;
@@ -66,15 +63,7 @@ int main(int argc, char** argv) {
             if (traced) CK(cudaMemset(dtrace, 0, 64 * (size_t)nbk * nbk));
             CK(cudaDeviceSynchronize());
             CK(cudaEventRecord(e0));
-            if (variant == 0) {
-                for (int k = 0; k < nbk; ++k) {
-                    chol_panel_kernel<<<std::max(1, (nbk - k - 1 + PANEL_WARPS - 1) / PANEL_WARPS), PANEL_WARPS * 32>>>(dA, npad, n, k, nbk, ddinv, dfail);
-                    const int T = nbk - k - 1;
-                    if (T > 0) chol_update_kernel<<<T * (T + 1) / 2, dim3(NB, NB)>>>(dA, npad, k, nbk);
-                }
-            } else if (variant == 1) chol_fused_kernel<false><<<grid, PANEL_WARPS * 32>>>(dA, npad, n, nbk, ntasks, ddinv, dfail, dready, ++epoch, dLinv, traced ? dtrace : nullptr);
-            else if (variant == 2) chol_fused_kernel<true><<<grid, PANEL_WARPS * 32>>>(dA, npad, n, nbk, ntasks, ddinv, dfail, dready, ++epoch, dLinv, traced ? dtrace : nullptr);
-            else chol_stream_kernel<<<grid, CS_THREADS>>>(dA, npad, n, nbk, ntasks, ddinv, dfail, dready, dprogress, ++epoch, dLinv, traced ? dtrace : nullptr);
+            chol_stream_kernel<<<grid, CS_THREADS>>>(dA, npad, n, nbk, ntasks, ddinv, dfail, dready, dprogress, ++epoch, dLinv, traced ? dtrace : nullptr);
             CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1)); CK(cudaGetLastError());
             float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
             if (rep >= 1 && !traced) { total += ms; best = std::min(best, ms); }
@@ -85,27 +74,23 @@ int main(int argc, char** argv) {
         for (int r = 0; r <= n; ++r) for (int c = 0; c <= std::min(r, n - 1); ++c) {
             err = std::max(err, std::fabs(out[(size_t)r * npad + c] - L[(size_t)r * npad + c])); ref = std::max(ref, std::fabs(L[(size_t)r * npad + c]));
         }
-        const char* name = variant == 0 ? "steps (panel+update kernels)" : variant == 1 ? "dataflow" : variant == 2 ? "dataflow + lookahead" : "streaming dataflow (DMMA updates)";
         printf("{\"variant\": \"%s\", \"cams\": %d, \"n\": %d, \"tile_rows\": %d, \"grid\": %d, \"tasks\": %d, \"avg_us\": %.1f, \"best_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_L\": %.3e, \"fail\": %d}\n",
-               name, nc, n, nbk, grid, ntasks, total / reps * 1e3, best * 1e3, err, ref, fail[0]);
-        if (variant == 0) continue;
+               "streaming dataflow (DMMA updates)", nc, n, nbk, grid, ntasks, total / reps * 1e3, best * 1e3, err, ref, fail[0]);
         CK(cudaMemcpy(tr.data(), dtrace, 64 * (size_t)ntasks, cudaMemcpyDeviceToHost));
         // critical path: per diagonal tile j, the stamps of the task that factors it
         unsigned long long t_start = ~0ull;
         for (int t = 0; t < ntasks; ++t) t_start = std::min(t_start, tr[(size_t)t * 8]);
         std::vector<double> pub(nbk, 0), seen(nbk, 0), solved(nbk, 0), pubx(nbk, 0), fact(nbk, 0), upd(nbk, 0), fstart(nbk, 0);
-        std::vector<double> sub_seen(nbk, 0), sub_solved(nbk, 0), sub_pub(nbk, 0);
         for (int t = 0; t < ntasks; ++t) {
             int i, c; bool merged;
-            if (variant == 1) decode<false>(t, nbk, i, c, merged); else decode<true>(t, nbk, i, c, merged);
+            decode(t, nbk, i, c, merged);
             const unsigned long long* e = &tr[(size_t)t * 8];
             auto us = [&](int slot) { return e[slot] ? (e[slot] - t_start) * 1e-3 : 0.0; };
             if (i == c || merged) { pub[i] = us(6); fact[i] = us(5); upd[i] = us(1); fstart[i] = us(7); }
             if (merged) { seen[i] = us(2); solved[i] = us(3); pubx[i] = us(4); }
-            if (variant == 1 && i == c + 1) { sub_seen[i] = us(2); sub_solved[i] = us(3); sub_pub[i] = us(4); }
         }
 #ifdef CHOL_FINE_TRACE
-        if (variant == 3) {
+        {
             unsigned long long f[64]; CK(cudaMemcpyFromSymbol(f, g_chol_fine, sizeof f));
             printf("  fine trace of the factorisation of tile 10 (cycles since entry): entry 0");
             for (int k = 1; k < 36; ++k) if (f[k]) printf("%s %lld", (k % 4) == 1 ? "\n    round owner_in/owner_out/after_barrier/[after_update]:" : "", (long long)(f[k] - f[0]));
@@ -117,23 +102,16 @@ int main(int argc, char** argv) {
 #endif
         printf("  j  published(j,j) us   step   | updates_done  diag_seen  solved  x_published  factor_start  factored\n");
         for (int j = 0; j < nbk; ++j) {
-            if (variant >= 2) printf("  %2d %10.2f %10.2f | %8.2f %8.2f %8.2f %8.2f %8.2f %8.2f\n", j, pub[j], j ? pub[j] - pub[j - 1] : pub[j], upd[j], seen[j], solved[j], pubx[j], fstart[j], fact[j]);
-            else printf("  %2d %10.2f %10.2f | %8.2f (sub-diagonal owner: seen %8.2f solved %8.2f published %8.2f) factored %8.2f\n", j, pub[j], j ? pub[j] - pub[j - 1] : pub[j], upd[j], sub_seen[j], sub_solved[j], sub_pub[j], fact[j]);
+            printf("  %2d %10.2f %10.2f | %8.2f %8.2f %8.2f %8.2f %8.2f %8.2f\n", j, pub[j], j ? pub[j] - pub[j - 1] : pub[j], upd[j], seen[j], solved[j], pubx[j], fstart[j], fact[j]);
         }
     }
-    // ---- back substitution variants on the factor left by the last run (Linv from the dataflow kernel)
+    // ---- both back substitutions on the factor left by the last run (Linv from the dataflow kernel)
     {
         std::vector<double> xr(n, 0.0), xg(n);
         for (int r = n - 1; r >= 0; --r) {
             double v = L[(size_t)n * npad + r];
             for (int k = r + 1; k < n; ++k) v -= L[(size_t)k * npad + r] * xr[k];
             xr[r] = v / L[(size_t)r * npad + r];
-        }
-        const size_t sm_staged = chol_backsolve_smem(npad, true), sm_plain = chol_backsolve_smem(npad, false);
-        const bool can_stage = sm_staged <= 220 * 1024;
-        if (can_stage) {
-            CK(cudaFuncSetAttribute(chol_backsolve_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_staged));
-            CK(cudaFuncSetAttribute(chol_backsolve_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_staged));
         }
         {   // cluster variant (BS_CLUSTER CTAs)
             const size_t cs = chol_backsolve_cluster_smem(n); const int cthreads = chol_backsolve_cluster_threads(n);
@@ -152,24 +130,20 @@ int main(int argc, char** argv) {
             int fl[4]; CK(cudaMemcpy(fl, dfail, 16, cudaMemcpyDeviceToHost));
             printf("{\"variant\": \"backsolve cluster of %d CTAs x %d threads, %zu B smem\", \"avg_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_x\": %.3e, \"fail\": %d}\n", BS_CLUSTER, cthreads, cs, total / reps * 1e3, err, ref, fl[0]);
         }
-        for (int v = 0; v < 4; ++v) {
-            const bool staged = v & 1, inv = v & 2;
-            if (staged && !can_stage) continue;
+        {   // single CTA
+            const size_t sm = chol_backsolve_smem(npad);
             float total = 0;
             for (int rep = 0; rep < reps + 1; ++rep) {
                 CK(cudaMemset(dx, 0, 8 * npad)); CK(cudaDeviceSynchronize());
                 CK(cudaEventRecord(e0));
-                if (staged && inv) chol_backsolve_kernel<true, true><<<1, 640, sm_staged>>>(dA, ddinv, dLinv, npad, n, dx);
-                else if (staged) chol_backsolve_kernel<true, false><<<1, 640, sm_staged>>>(dA, ddinv, dLinv, npad, n, dx);
-                else if (inv) chol_backsolve_kernel<false, true><<<1, 640, sm_plain>>>(dA, ddinv, dLinv, npad, n, dx);
-                else chol_backsolve_kernel<false, false><<<1, 640, sm_plain>>>(dA, ddinv, dLinv, npad, n, dx);
+                chol_backsolve_kernel<<<1, 640, sm>>>(dA, dLinv, npad, n, dx);
                 CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1)); CK(cudaGetLastError());
                 float ms; CK(cudaEventElapsedTime(&ms, e0, e1)); if (rep) total += ms;
             }
             CK(cudaMemcpy(xg.data(), dx, 8 * n, cudaMemcpyDeviceToHost));
             double err = 0, ref = 0;
             for (int r = 0; r < n; ++r) { err = std::max(err, std::fabs(xg[r] - xr[r])); ref = std::max(ref, std::fabs(xr[r])); }
-            printf("{\"variant\": \"backsolve staged=%d inverse_tiles=%d\", \"avg_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_x\": %.3e}\n", (int)staged, (int)inv, total / reps * 1e3, err, ref);
+            printf("{\"variant\": \"backsolve single CTA x 640 threads, %zu B smem\", \"avg_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_x\": %.3e}\n", sm, total / reps * 1e3, err, ref);
         }
     }
     return 0;
