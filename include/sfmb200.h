@@ -397,6 +397,32 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
                               const size_t* out_stride);
 int sfmb200_jpeg_last_stats(const sfmb200_ctx* ctx, int64_t* stats7);
 
+/* ---- f-3: image downscale, the optional step after imread -------------------------------------------------------- */
+/*
+ * The downscale of SfM::setImagesDirectory (SfM.cpp:127-129, main.cpp's -s/--downscale):
+ *     if (mDownscaleFactor != 1.0) resize(img, img, Size(), mDownscaleFactor, mDownscaleFactor);
+ * byte-identical to OpenCV 4.13's cv::resize with the default INTER_LINEAR on 8-bit B,G,R images.  `scale` is the reference's float
+ * factor widened to double.  Output size cvRound(w * scale) x cvRound(h * scale) (half to even: 173 * 0.5 -> 86, 175 * 0.5 -> 88).
+ * A factor of exactly 0.5 takes OpenCV's 2x2 area path; any other factor its Q11 fixed-point bilinear path; an image whose size does
+ * not change is copied, and a factor of exactly 1 returns the input bytes (the reference does not call resize then).  A scale that is
+ * not finite or <= 0, or that leaves an image with no pixels, returns SFMB200_ERR_INVALID (cv::resize asserts).
+ *
+ * sfmb200_resize_size: host only (no context, no GPU): the output size of a w x h image.
+ * sfmb200_resize_batch: resizes the n host images src[i] (w[i] x h[i], B,G,R, rows of src_stride[i] bytes) into caller-owned host
+ * buffers dst[i] sized with sfmb200_resize_size, rows of dst_stride[i] bytes (a stride array NULL or an entry 0 = packed rows).  The
+ * images may differ in size.  One upload, one launch, one download and one host synchronisation per call; a factor of 1 copies on
+ * the host.  At most 65535 images per call.
+ * sfmb200_decode_jpeg_batch_scaled: sfmb200_decode_jpeg_batch followed by the downscale on the device, in one call: only the resized
+ * images are downloaded (sfmb200_jpeg_last_stats [6] counts them).  Each out_bgr[i] holds the size sfmb200_resize_size gives for the
+ * size sfmb200_jpeg_info reports; out_stride as in sfmb200_decode_jpeg_batch.  scale == 1 returns exactly the bytes of
+ * sfmb200_decode_jpeg_batch.
+ */
+int sfmb200_resize_size(int w, int h, double scale, int* dw, int* dh);
+int sfmb200_resize_batch(sfmb200_ctx* ctx, const uint8_t* const* src, const int* w, const int* h, const size_t* src_stride, int n,
+                         double scale, uint8_t* const* dst, const size_t* dst_stride);
+int sfmb200_decode_jpeg_batch_scaled(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale,
+                                     uint8_t* const* out_bgr, const size_t* out_stride);
+
 /* ---- multi-GPU plumbing (NCCL, one process per GPU) ------------------------------------------------------ */
 #define SFMB200_UNIQUE_ID_BYTES 128
 int sfmb200_comm_unique_id(uint8_t* id /* [SFMB200_UNIQUE_ID_BYTES] */);       /* rank 0, then broadcast by the host */

@@ -366,22 +366,55 @@ class Context:
         """sfmb200_jpeg_info (host only): (status, width, height, components) of a JPEG file given as bytes."""
         return jpeg_info(data)
 
-    def decode_jpeg(self, files):
+    def decode_jpeg(self, files, scale=1.0):
         """sfmb200_decode_jpeg_batch: `files` is a list of JPEG files as bytes; returns a list of uint8 [h, w, 3] B,G,R images,
         byte-identical to cv2.imdecode(buf, IMREAD_COLOR), in one call.  Raises SfmB200Error (naming the file) if any file is
-        unsupported (status 5) or corrupt (status 1)."""
+        unsupported (status 5) or corrupt (status 1).  With scale != 1 (sfmb200_decode_jpeg_batch_scaled) every image is also
+        downscaled on the device, byte-identical to cv2.resize(img, None, fx=scale, fy=scale), and only the resized images are
+        downloaded."""
         files = [bytes(f) for f in files]
         n = len(files)
+        scale = float(scale)
         if n == 0:
             return []
         outs = []
         for f in files:
             rc, w, h, _ = jpeg_info(f)
+            if rc == 0 and scale != 1.0:
+                w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
             outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
         data = (C.c_char_p * n)(*files)
         sizes = (C.c_size_t * n)(*[len(f) for f in files])
         ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        self._check(lib().sfmb200_decode_jpeg_batch(self._h, data, sizes, n, ptrs, None))
+        if scale == 1.0:
+            self._check(lib().sfmb200_decode_jpeg_batch(self._h, data, sizes, n, ptrs, None))
+        else:
+            self._check(lib().sfmb200_decode_jpeg_batch_scaled(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
+        return outs
+
+    def resize_images(self, images, scale):
+        """sfmb200_resize_batch: `images` is a list of uint8 [h, w, 3] B,G,R arrays (any sizes, strided rows allowed); returns them
+        resized by `scale`, byte-identical to cv2.resize(img, None, fx=scale, fy=scale) (INTER_LINEAR), in one call.  A refused scale
+        raises SfmB200Error (status 1)."""
+        n = len(images)
+        if n == 0:
+            return []
+        srcs, outs = [], []
+        for im in images:
+            im = np.asarray(im)
+            if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError("resize_images: expects uint8 [h, w, 3] B,G,R images")
+            if im.strides[1:] != (3, 1) or im.strides[0] < 3 * im.shape[1]:
+                im = np.ascontiguousarray(im)                    # pixels packed B,G,R; rows may keep a longer stride
+            srcs.append(im)
+            h, w = im.shape[:2]
+            dw, dh = resize_size(w, h, scale) or (1, 1)          # a refused scale fails the call below
+            outs.append(np.empty((dh, dw, 3), np.uint8))
+        ptr = (C.c_void_p * n)(*[s.ctypes.data for s in srcs])
+        ws = (C.c_int * n)(*[s.shape[1] for s in srcs]); hs = (C.c_int * n)(*[s.shape[0] for s in srcs])
+        strides = (C.c_size_t * n)(*[s.strides[0] for s in srcs])
+        dptr = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        self._check(lib().sfmb200_resize_batch(self._h, ptr, ws, hs, strides, n, C.c_double(float(scale)), dptr, None))
         return outs
 
     def jpeg_last_stats(self):
@@ -432,6 +465,14 @@ def jpeg_info(data):
     w = C.c_int(0); h = C.c_int(0); c = C.c_int(0)
     rc = lib().sfmb200_jpeg_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(c))
     return int(rc), w.value, h.value, c.value
+
+
+def resize_size(width, height, scale):
+    """sfmb200_resize_size: (width, height) of cv2.resize(img, None, fx=scale, fy=scale) for a width x height image, without a
+    context or a GPU; None where cv::resize refuses (scale not finite or <= 0, or no pixels left)."""
+    w = C.c_int(0); h = C.c_int(0)
+    rc = lib().sfmb200_resize_size(int(width), int(height), C.c_double(float(scale)), C.byref(w), C.byref(h))
+    return (w.value, h.value) if rc == 0 else None
 
 
 def comm_unique_id():

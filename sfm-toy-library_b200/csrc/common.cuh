@@ -128,6 +128,8 @@ struct sfmb200_ctx {
     DevBuf jpeg_dev;                    // JPEG decoding (jpeg.cu): tables, entropy data, coefficients, planes, images of the last batch
     PinBuf jpeg_pin_up, jpeg_pin_down;  // its one upload and its one download
     int64_t jpeg_stats[7] = {0, 0, 0, 0, 0, 0, 0};   // sfmb200_jpeg_last_stats of the last batch
+    DevBuf rz_dev;                      // image downscale (resize.cu): descriptors, taps, source and resized images of the last batch
+    PinBuf rz_pin_up, rz_pin_down;      // its one upload and its one download
 };
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);
@@ -156,3 +158,11 @@ int sfmb200_allreduce_sum_f64(sfmb200_ctx* ctx, double* dbuf, size_t n);
 int sfmb200_allreduce_max_f64(sfmb200_ctx* ctx, double* dbuf, size_t n);
 int sfmb200_allgather_bytes(sfmb200_ctx* ctx, const void* d_send, void* d_recv, size_t bytes);
 void sfmb200_comm_destroy(sfmb200_ctx* ctx);
+
+// image downscale (resize.cu), also run by the scaled JPEG decode (jpeg.cu) on the images it has just decoded.
+// rz_plan: fills dw, dh, the tap offsets and the tiles of imgs[0..n) (sw, sh set by the caller) and appends their taps; false and the
+// image in *bad if a size is refused.  rz_enqueue: one launch on ctx->stream over device copies of imgs / taps.
+struct RzImg; struct RzTap;
+bool rz_plan(double scale, RzImg* imgs, int n, std::vector<RzTap>& taps, int* bad);
+int rz_enqueue(sfmb200_ctx* ctx, double scale, const RzImg* imgs, int n, const RzImg* d_imgs, const RzTap* d_taps, const uint8_t* d_src,
+               uint8_t* d_dst);

@@ -11,9 +11,12 @@
 //   jd_dc_sum + scan + jd_dc_apply   DC prediction: per-component prefix sums over MCUs, reset at every restart segment
 //   jd_idct           dequantisation and jpeg_idct_islow, 8 threads per block, into uint8 component planes
 //   jd_color          upsampling, YCbCr -> B,G,R and the EXIF orientation, into the download area
+//   rz_*              (sfmb200_decode_jpeg_batch_scaled only) jd_color writes to device memory and the downscale of resize.cu
+//                     writes the resized images into the download area instead
 // then one download (per-image error flags, statistics and the images) and one host synchronisation.
 #include "common.cuh"
 #include "jpeg_parse.h"
+#include "resize_math.cuh"
 
 namespace {
 
@@ -345,29 +348,16 @@ size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 }  // namespace
 
-extern "C" {
-
-int sfmb200_jpeg_info(const uint8_t* data, size_t size, int* width, int* height, int* components) {
-    JpImage im; std::string why;
-    const int rc = jp_parse(data, size, JD_CHUNK, im, why);
-    if (rc) return rc;
-    if (width) *width = im.OW;
-    if (height) *height = im.OH;
-    if (components) *components = im.ncomp;
-    return SFMB200_OK;
-}
-
-int sfmb200_jpeg_last_stats(const sfmb200_ctx* ctx, int64_t* stats7) {
-    if (!ctx || !stats7) return SFMB200_ERR_INVALID;
-    for (int i = 0; i < 7; ++i) stats7[i] = ctx->jpeg_stats[i];
-    return SFMB200_OK;
-}
-
-int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, uint8_t* const* out_bgr,
-                              const size_t* out_stride) {
+// Both decode entry points.  scale == 1: jd_color writes the images into the download area.  Otherwise jd_color writes them to device
+// memory, resize.cu's kernels downscale them into the download area, and only the resized images come back.
+static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
+                     const size_t* out_stride) {
     if (!ctx) return SFMB200_ERR_INVALID;
     if (n < 0 || (n > 0 && (!data || !size || !out_bgr))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: bad arguments");
     if (n > 65535) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: at most 65535 images per call");
+    if (!std::isfinite(scale) || scale <= 0)
+        return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch_scaled: scale %g is not a positive finite number", scale);
+    const bool scaled = scale != 1.0;
     for (int i = 0; i < 7; ++i) ctx->jpeg_stats[i] = 0;
     if (n == 0) return SFMB200_OK;
     SFM_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -382,8 +372,20 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     for (int i = 0; i < n; ++i) {
         if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", i, whys[i].c_str());
         if (!out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", i);
-        if (out_stride && out_stride[i] && out_stride[i] < (size_t)ims[i].OW * 3)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", i, out_stride[i], ims[i].OW * 3);
+    }
+    // ---- the downscale: output sizes and taps of every image
+    std::vector<RzImg> rz(scaled ? n : 0);
+    std::vector<RzTap> taps;
+    if (scaled) {
+        for (int i = 0; i < n; ++i) { memset(&rz[i], 0, sizeof(RzImg)); rz[i].sw = ims[i].OW; rz[i].sh = ims[i].OH; }
+        int bad = 0;
+        if (!rz_plan(scale, rz.data(), n, taps, &bad))
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", bad, scale, ims[bad].OW, ims[bad].OH);
+    }
+    for (int i = 0; i < n; ++i) {
+        const int ow = scaled ? rz[i].dw : ims[i].OW;
+        if (out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", i, out_stride[i], ow * 3);
     }
 
     // ---- layout
@@ -392,7 +394,7 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     std::vector<JdChunk> chunks;
     std::vector<size_t> in0(n);
     size_t in_bytes = 0, ubytes = 0;
-    long long blocks = 0, mcus = 0, planes = 0, outb = 0;
+    long long blocks = 0, mcus = 0, planes = 0, outb = 0, rzb = 0;    // outb: decoded images; rzb: resized images
     for (int i = 0; i < n; ++i) {
         const JpImage& p = ims[i];
         JdImg& d = img[i];
@@ -406,6 +408,11 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
         }
         d.nblocks = blocks - d.blk0[0];
         d.out0 = outb; outb += (long long)al256((size_t)p.OW * p.OH * 3);
+        if (scaled) {
+            RzImg& r = rz[i];
+            r.src0 = d.out0; r.src_stride = (long long)p.OW * 3;
+            r.dst0 = rzb; r.dst_stride = (long long)r.dw * 3; rzb += (long long)al256((size_t)r.dst_stride * r.dh);
+        }
         d.mcu0 = mcus; d.nmcu = p.mcus(); mcus += d.nmcu;
         d.scan = p.scan; d.tab0 = 8 * i;
         // chunks of the scan (aligned, so that every chunk belongs to one image) and the unstuffed positions
@@ -444,7 +451,8 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     const size_t o_tabs = 0, o_qt = o_tabs + al256(sizeof(JmHuff) * 8 * n), o_img = o_qt + al256(sizeof(int16_t) * 192 * n);
     const size_t o_seg = o_img + al256(sizeof(JdImg) * n), o_sub = o_seg + al256(sizeof(JdSeg) * nseg);
     const size_t o_chunk = o_sub + al256(sizeof(int) * nsub), o_in = o_chunk + al256(sizeof(JdChunk) * nchunk);
-    const size_t up_bytes = o_in + al256(in_bytes + 8);
+    const size_t o_rzimg = o_in + al256(in_bytes + 8), o_rztap = o_rzimg + al256(sizeof(RzImg) * rz.size());
+    const size_t up_bytes = o_rztap + al256(sizeof(RzTap) * taps.size());
     SFM_CUDA(ctx, ctx->jpeg_pin_up.reserve(up_bytes));
     char* up = (char*)ctx->jpeg_pin_up.p;
     pool.parallel_for(n, [&](int i) {
@@ -457,18 +465,23 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     memcpy(up + o_sub, sub_seg.data(), sizeof(int) * nsub);
     memcpy(up + o_chunk, chunks.data(), sizeof(JdChunk) * nchunk);
     memset(up + o_in + in_bytes, 0, 8);
+    if (scaled) {
+        memcpy(up + o_rzimg, rz.data(), sizeof(RzImg) * n);
+        memcpy(up + o_rztap, taps.data(), sizeof(RzTap) * taps.size());
+    }
 
     // ---- device memory
     const size_t o_down = al256(up_bytes);
     const size_t o_err = 0, o_stats = al256(sizeof(int) * n), o_out = o_stats + al256(sizeof(JdStats));
-    const size_t down_bytes = o_out + (size_t)outb;
+    const size_t down_bytes = o_out + (size_t)(scaled ? rzb : outb);
     const size_t o_u = o_down + al256(down_bytes), o_exit = o_u + al256(ubytes + 16);
     const size_t o_comp = o_exit + al256(8ull * nsub), o_chg = o_comp + al256(4ull * nsub), o_nblk = o_chg + al256(4ull * nsub);
     const size_t o_pre = o_nblk + al256(4ull * nsub), o_part = o_pre + al256(4ull * nsub);
     const size_t o_rc = o_part + al256(8ull * (ceil_div64(std::max<long long>(nsub, mcus), SCAN_TILE) + 1));
     const size_t o_msum = o_rc + 256, o_mpre = o_msum + al256(8ull * mcus);
     const size_t o_coef = o_mpre + al256(8ull * mcus), o_planes = o_coef + al256(128ull * blocks);
-    const size_t total = o_planes + al256((size_t)planes);
+    const size_t o_full = o_planes + al256((size_t)planes);          // the decoded images of a scaled call (not downloaded)
+    const size_t total = o_full + (scaled ? (size_t)outb : 0);
     SFM_CUDA(ctx, ctx->jpeg_dev.reserve(total));
     char* dv = (char*)ctx->jpeg_dev.p;
     const JmHuff* d_tabs = (const JmHuff*)(dv + o_tabs);
@@ -491,6 +504,7 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     unsigned long long* d_msum = (unsigned long long*)(dv + o_msum); unsigned long long* d_mpre = (unsigned long long*)(dv + o_mpre);
     int16_t* d_coef = (int16_t*)(dv + o_coef);
     uint8_t* d_planes = (uint8_t*)(dv + o_planes);
+    uint8_t* d_full = scaled ? (uint8_t*)(dv + o_full) : d_out;
     cudaStream_t st = ctx->stream;
 
     SFM_CUDA(ctx, cudaMemcpyAsync(dv, up, up_bytes, cudaMemcpyHostToDevice, st));
@@ -524,8 +538,10 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
     SFM_LAUNCH_CHECK(ctx);
     jd_idct<<<dim3((unsigned)ceil_div64(max_blk, 32), (unsigned)n), 256, 0, st>>>(d_img, d_coef, d_qt, d_planes);
     SFM_LAUNCH_CHECK(ctx);
-    jd_color<<<dim3((unsigned)ceil_div64(max_pix, 256), (unsigned)n), 256, 0, st>>>(d_img, d_planes, d_out);
+    jd_color<<<dim3((unsigned)ceil_div64(max_pix, 256), (unsigned)n), 256, 0, st>>>(d_img, d_planes, d_full);
     SFM_LAUNCH_CHECK(ctx);
+    if (scaled)
+        if (int rc = rz_enqueue(ctx, scale, rz.data(), n, (const RzImg*)(dv + o_rzimg), (const RzTap*)(dv + o_rztap), d_full, d_out)) return rc;
     SFM_CUDA(ctx, ctx->jpeg_pin_down.reserve(down_bytes));
     char* hd = (char*)ctx->jpeg_pin_down.p;
     SFM_CUDA(ctx, cudaMemcpyAsync(hd, down, down_bytes, cudaMemcpyDeviceToHost, st));
@@ -542,12 +558,41 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
                                 herr[i] & JD_ERR_DATA ? "corrupt entropy-coded data (no Huffman code, overrun or a run past coefficient 63)"
                                                       : "entropy-coded data ends before the last block");
     pool.parallel_for(n, [&](int i) {
-        const size_t row = (size_t)img[i].OW * 3, stride = out_stride && out_stride[i] ? out_stride[i] : row;
-        const uint8_t* src = (const uint8_t*)(hd + o_out + img[i].out0);
-        if (stride == row) memcpy(out_bgr[i], src, row * img[i].OH);
-        else for (int y = 0; y < img[i].OH; ++y) memcpy(out_bgr[i] + y * stride, src + y * row, row);
+        const int ow = scaled ? rz[i].dw : img[i].OW, oh = scaled ? rz[i].dh : img[i].OH;
+        const size_t row = (size_t)ow * 3, stride = out_stride && out_stride[i] ? out_stride[i] : row;
+        const uint8_t* src = (const uint8_t*)(hd + o_out + (scaled ? rz[i].dst0 : img[i].out0));
+        if (stride == row) memcpy(out_bgr[i], src, row * oh);
+        else for (int y = 0; y < oh; ++y) memcpy(out_bgr[i] + y * stride, src + y * row, row);
     });
     return SFMB200_OK;
+}
+
+extern "C" {
+
+int sfmb200_jpeg_info(const uint8_t* data, size_t size, int* width, int* height, int* components) {
+    JpImage im; std::string why;
+    const int rc = jp_parse(data, size, JD_CHUNK, im, why);
+    if (rc) return rc;
+    if (width) *width = im.OW;
+    if (height) *height = im.OH;
+    if (components) *components = im.ncomp;
+    return SFMB200_OK;
+}
+
+int sfmb200_jpeg_last_stats(const sfmb200_ctx* ctx, int64_t* stats7) {
+    if (!ctx || !stats7) return SFMB200_ERR_INVALID;
+    for (int i = 0; i < 7; ++i) stats7[i] = ctx->jpeg_stats[i];
+    return SFMB200_OK;
+}
+
+int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, uint8_t* const* out_bgr,
+                              const size_t* out_stride) {
+    return jd_decode(ctx, data, size, n, 1.0, out_bgr, out_stride);
+}
+
+int sfmb200_decode_jpeg_batch_scaled(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale,
+                                     uint8_t* const* out_bgr, const size_t* out_stride) {
+    return jd_decode(ctx, data, size, n, scale, out_bgr, out_stride);
 }
 
 }  // extern "C"

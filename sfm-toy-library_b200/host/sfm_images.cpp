@@ -1,4 +1,5 @@
-// sfm_images.cpp -- sfmtoylib::readImages (sfm_images.h) over sfmb200_jpeg_info / sfmb200_decode_jpeg_batch.
+// sfm_images.cpp -- sfmtoylib::readImages (sfm_images.h) over sfmb200_jpeg_info / sfmb200_decode_jpeg_batch, or with a downscale
+// sfmb200_resize_size / sfmb200_decode_jpeg_batch_scaled.
 #include "sfm_images.h"
 #include "../../include/sfmb200.h"
 
@@ -34,7 +35,8 @@ sfmb200_ctx* context() {
 
 }  // namespace
 
-bool readImages(const std::vector<std::string>& filenames, std::vector<cv::Mat>& images) {
+bool readImages(const std::vector<std::string>& filenames, std::vector<cv::Mat>& images, float downscale) {
+    const double scale = downscale;      // the reference's float factor, widened as cv::resize receives it
     std::vector<std::vector<uint8_t>> files(filenames.size());
     std::vector<const uint8_t*> data(files.size());
     std::vector<size_t> size(files.size());
@@ -50,12 +52,18 @@ bool readImages(const std::vector<std::string>& filenames, std::vector<cv::Mat>&
             std::cerr << "Unable to read image from file: " << filenames[i] << " (not a JPEG file the GPU decoder supports)" << std::endl;
             return false;
         }
+        if (scale != 1.0 && sfmb200_resize_size(w, h, scale, &w, &h) != SFMB200_OK) {
+            std::cerr << "Unable to downscale image " << filenames[i] << " by " << downscale << std::endl;
+            return false;
+        }
         out[i] = cv::Mat(h, w, kType8UC3);
         dst[i] = out[i].data;
     }
     sfmb200_ctx* ctx = context();
     if (!ctx) return false;
-    if (sfmb200_decode_jpeg_batch(ctx, data.data(), size.data(), (int)files.size(), dst.data(), nullptr) != SFMB200_OK) {
+    const int rc = scale == 1.0 ? sfmb200_decode_jpeg_batch(ctx, data.data(), size.data(), (int)files.size(), dst.data(), nullptr)
+                                : sfmb200_decode_jpeg_batch_scaled(ctx, data.data(), size.data(), (int)files.size(), scale, dst.data(), nullptr);
+    if (rc != SFMB200_OK) {
         std::cerr << "sfmb200: decode_jpeg_batch: " << sfmb200_last_error(ctx) << std::endl;
         return false;
     }

@@ -129,10 +129,13 @@ class SfM:
         return sfm
 
     @classmethod
-    def from_directory(cls, path, readImages: Callable = None, extractAllFeatures: Callable = None, **kw):
+    def from_directory(cls, path, readImages: Callable = None, extractAllFeatures: Callable = None, *, downscale: float = 1.0, **kw):
         """SfM::setImagesDirectory (SfM.cpp:97-139): the .jpg / .png files of `path` (extension compared case-insensitively), sorted
         by name, read by the injected stage (default cv2.imread per file; stages.readImages decodes them all on the device), then
-        from_images.  The reference's optional downscale (:127-129) is not applied."""
+        from_images.  With downscale != 1 (main.cpp's -s) every image is resized as at :127-129, byte-identical to cv::resize: an
+        injected readImages is called as readImages(files, downscale=...) and resizes in the same call (stages.readImages does so on
+        the device); after cv2.imread, stages.resizeImages resizes them all in one device call.  K then follows from the
+        downscaled size (SfM.cpp:70-72)."""
         import os
         names = sorted(f for f in os.listdir(path) if os.path.splitext(f)[1].lower() in (".jpg", ".png"))
         if not names:
@@ -142,12 +145,17 @@ class SfM:
         if readImages is None:
             import cv2
             images = [cv2.imread(f) for f in files]
+        elif float(np.float32(downscale)) != 1.0:
+            images = list(readImages(files, downscale=downscale))
         else:
             images = list(readImages(files))
         dt = time.perf_counter() - t0
         for f, im in zip(files, images):
             if im is None or im.size == 0:
                 raise ValueError(f"Unable to read image from file: {f}")
+        if readImages is None and float(np.float32(downscale)) != 1.0:
+            images = stages.resizeImages(images, downscale)
+            dt = time.perf_counter() - t0
         sfm = cls.from_images(images, extractAllFeatures, **kw)
         sfm.seconds["read"] = dt; sfm.calls["read"] = len(files)
         return sfm

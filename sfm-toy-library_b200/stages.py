@@ -64,16 +64,33 @@ def GetAlignedMatching(size):          # SfMCommon.cpp:120-126
     return m
 
 
-def readImages(files: List[str], ctx=None) -> List[np.ndarray]:
+def _reference_factor(downscale) -> float:
+    """The reference keeps the factor as `float mDownscaleFactor` (SfM.h) and passes it to cv::resize widened to double."""
+    return float(np.float32(downscale))
+
+
+def readImages(files: List[str], ctx=None, downscale: float = 1.0) -> List[np.ndarray]:
     """The imread loop of SfM::setImagesDirectory (SfM.cpp:123-135) on the device: every file decoded in one
-    sfmb200_decode_jpeg_batch call, byte-identical to cv2.imread(file) (B,G,R, EXIF orientation applied).  Only JPEG files decode
-    (there is no host fallback): any other file raises capi.SfmB200Error naming it."""
+    sfmb200_decode_jpeg_batch call, byte-identical to cv2.imread(file) (B,G,R, EXIF orientation applied).  With downscale != 1 the
+    loop's resize (:127-129) runs on the device in the same call (sfmb200_decode_jpeg_batch_scaled), byte-identical to
+    cv2.resize(cv2.imread(file), None, fx=s, fy=s) with s the factor as the reference's float.  Only JPEG files decode (there is
+    no host fallback): any other file raises capi.SfmB200Error naming it."""
     ctx = ctx or default_context()
     blobs = []
     for f in files:
         with open(f, "rb") as fh:
             blobs.append(fh.read())
-    return ctx.decode_jpeg(blobs)
+    return ctx.decode_jpeg(blobs, _reference_factor(downscale))
+
+
+def resizeImages(images: List[np.ndarray], downscale: float, ctx=None) -> List[np.ndarray]:
+    """The resize of SfM::setImagesDirectory (SfM.cpp:127-129) for images already in host memory (PNG files, cv2.imread):
+    all of them in one sfmb200_resize_batch call, byte-identical to cv2.resize(img, None, fx=s, fy=s) with s the factor as the
+    reference's float.  A factor of 1 returns the images unchanged, as the reference skips the call."""
+    s = _reference_factor(downscale)
+    if s == 1.0:
+        return list(images)
+    return (ctx or default_context()).resize_images(list(images), s)
 
 
 ORB_FEATURES = 5000                    # mDetector = ORB::create(5000), SfM2DFeatureUtilities.cpp:39
