@@ -277,9 +277,32 @@ int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* 
  * E [ns][10][9] (unit Frobenius norm, real roots in ascending order), nsol [ns].
  * sfmb200_essential_last_trace: the last sfmb200_find_camera_matrices call's samples [cap][5], solution counts nsol [cap] and
  * per-solution inlier counts [cap * 10] in (sample, solution) order, for its first min(cap, n_samples) samples; any output may
- * be NULL.  Returns that call's n_samples (0 before any call), or -1 on bad arguments. */
+ * be NULL.  Returns that call's n_samples (0 before any call), or -1 on bad arguments.  After a
+ * sfmb200_find_camera_matrices_pairs call it describes that call's pair if it had exactly one, and returns 0 otherwise. */
 int sfmb200_five_point(sfmb200_ctx* ctx, const double* x1, const double* x2, int ns, double* E, int32_t* nsol);
 int sfmb200_essential_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, int32_t* nsol, int32_t* counts);
+/*
+ * sfmb200_find_camera_matrices for every pair of a batch in one call, with the input layout of sfmb200_find_homography_pairs
+ * (pts / img_off / pairs / match_q / match_t / match_off below), so one set of arrays serves both calls.  Pair p's outputs
+ * (E, R, t, its slices of both masks, summary[p]) are bitwise what sfmb200_find_camera_matrices returns for that pair's matches
+ * with the same options, whatever else is in the batch and wherever the pair stands in it: one seed covers the call and every
+ * pair draws its samples from it as a single call does.  Per pair as in the single call: m < 5 gives found = 0 and zeros, m == 5
+ * one sample, no model found = 0 with zeros.
+ *   K [9] float row-major, shared by all pairs.  pts [img_off[n_img] * 2]: key points of all images; img_off [n_img + 1]
+ *   monotone from 0; pairs [n_pairs * 2] (left, right) image; pair p owns matches match_off[p] .. match_off[p+1] (match_q /
+ *   match_t index the left / right image's key points; match_off [n_pairs + 1] monotone from 0).
+ *   E [n_pairs * 9], R [n_pairs * 9], t [n_pairs * 3]: any may be NULL.  inlier_mask / pose_mask [match_off[n_pairs]]: either
+ *   may be NULL.  summary [n_pairs]: may be NULL.  opt NULL = defaults.
+ * Inputs are checked on the host before any launch: an image index out of range, non-monotone offsets, match_off[0] != 0, a match
+ * index outside its image and the option / K checks of the single call give SFMB200_ERR_INVALID with a message, and the context
+ * stays usable.  n_pairs == 0 does nothing.  One upload, one download, one host synchronisation per call.  The pairs run in
+ * consecutive groups whose hypotheses (10 x 96 B per sample, 0.96 MB per pair at max_iters 1000) fit 256 MB of device memory,
+ * enqueued back to back.
+ */
+int sfmb200_find_camera_matrices_pairs(sfmb200_ctx* ctx, const float* K, const float* pts, const int32_t* img_off, int n_img,
+                                       const int32_t* pairs, int n_pairs, const int32_t* match_q, const int32_t* match_t,
+                                       const int64_t* match_off, const sfmb200_essential_options* opt, double* E, double* R, double* t,
+                                       uint8_t* inlier_mask, uint8_t* pose_mask, sfmb200_essential_summary* summary);
 
 /* ---- f-2: homography RANSAC for many image pairs, all on the device -------------------------------------------- */
 /*

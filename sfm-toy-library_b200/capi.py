@@ -246,6 +246,32 @@ class Context:
                                                        _p(Rm, C.c_double), _p(t, C.c_double), _p(inl, C.c_uint8), _p(pm, C.c_uint8), C.byref(s)))
         return E.reshape(3, 3), Rm.reshape(3, 3), t, inl[:m], pm[:m], s.as_dict()
 
+    def find_camera_matrices_pairs(self, K, points, pairs, match_q, match_t, match_off, options=None, **kw):
+        """sfmb200_find_camera_matrices_pairs: find_camera_matrices for every pair in one call, with the arguments of
+        find_homography_pairs (points: list of [n_i, 2] key points per image; pairs [P, 2]; match_q / match_t: all pairs' matches
+        concatenated, pair p owning match_off[p]:match_off[p+1]).  options: EssentialOptions or keyword overrides of the defaults.
+        Returns (E [P, 3, 3], R [P, 3, 3], t [P, 3], inlier_mask [sum of matches], pose_mask [sum of matches], summary dict of
+        arrays found / n_inliers / n_good / iterations / n_samples / n_hypotheses [P])."""
+        K = np.ascontiguousarray(K, np.float32).reshape(9)
+        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
+        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
+        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
+        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
+        moff = np.ascontiguousarray(match_off, np.int64)
+        P = pairs.shape[0]
+        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
+            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+        o = options or essential_default_options(**kw)
+        E = np.zeros((max(P, 1), 9)); Rm = np.zeros((max(P, 1), 9)); t = np.zeros((max(P, 1), 3))
+        inl = np.zeros(max(mq.shape[0], 1), np.uint8); pm = np.zeros(max(mq.shape[0], 1), np.uint8); s = (EssentialSummary * max(P, 1))()
+        self._check(lib().sfmb200_find_camera_matrices_pairs(self._h, _p(K, C.c_float), _p(allp, C.c_float), _p(img_off, C.c_int32), len(pts),
+                                                             _p(pairs, C.c_int32), P, _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64),
+                                                             C.byref(o), _p(E, C.c_double), _p(Rm, C.c_double), _p(t, C.c_double),
+                                                             _p(inl, C.c_uint8), _p(pm, C.c_uint8), s))
+        summ = {k: np.array([getattr(s[p], k) for p in range(P)], np.int32) for k, _ in EssentialSummary._fields_}
+        return E[:P].reshape(P, 3, 3), Rm[:P].reshape(P, 3, 3), t[:P], inl[:mq.shape[0]], pm[:mq.shape[0]], summ
+
     def five_point(self, x1, x2):
         """sfmb200_five_point: x1, x2 [ns, 5, 2] normalised coordinates -> (E [ns, 10, 3, 3], nsol [ns])."""
         x1 = np.ascontiguousarray(x1, np.float64).reshape(-1, 5, 2); x2 = np.ascontiguousarray(x2, np.float64).reshape(-1, 5, 2)

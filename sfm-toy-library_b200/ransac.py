@@ -126,6 +126,28 @@ def findCameraMatricesFromMatch_gpu(intrinsics: Intrinsics, matches, left: Featu
     return True, matches[pose_mask != 0].copy(), Pleft, Pright
 
 
+def cameraMatricesManyPairs(intrinsics: Intrinsics, features, pairs, matches, ctx=None, seed=0):
+    """findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) for every pair in one device call
+    (sfmb200_find_camera_matrices_pairs).  features: per image Features; pairs [(i, j), ...]; matches: per pair a structured array
+    with queryIdx / trainIdx.  Returns one (success, prunedMatches, Pleft, Pright) per pair, each exactly what
+    findCameraMatricesFromMatch_gpu returns for that pair with the same seed."""
+    ctx = ctx or default_context()
+    if len(pairs) == 0:
+        return []
+    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
+    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
+    _, R, t, _, pose_mask, s = ctx.find_camera_matrices_pairs(intrinsics.K, [f.points for f in features], pairs, mq, mt, off, seed=seed)
+    out = []
+    for p, m in enumerate(matches):
+        Pleft = np.eye(3, 4, dtype=np.float32)
+        if not s["found"][p]:
+            out.append((False, m[:0].copy(), Pleft, Pleft.copy()))
+            continue
+        Pright = np.concatenate([R[p], t[p].reshape(3, 1)], 1).astype(np.float32)
+        out.append((True, m[pose_mask[off[p]:off[p + 1]] != 0].copy(), Pleft, Pright))
+    return out
+
+
 def findCameraPoseFrom2D3DMatch(intrinsics: Intrinsics, points2D, points3D, ctx=None, iterations=100, seed=0):
     """SfMStereoUtilities::findCameraPoseFrom2D3DMatch (SfMStereoUtilities.cpp:208-243).  Returns (success, pose 3x4 float32)."""
     import cv2

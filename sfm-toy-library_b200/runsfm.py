@@ -93,7 +93,8 @@ class SfM:
     def __init__(self, features: List[Features], image_size, *, matchFeatures: Callable = None, triangulateViews: Callable = None,
                  adjustBundle: Callable = None, matchAllPairs: Callable = None, findHomographyInliers: Callable = None,
                  findCameraMatricesFromMatch: Callable = None, findCameraPoseFrom2D3DMatch: Callable = None,
-                 homographyInliersAllPairs: Callable = None, trace: Optional[list] = None, verbose: bool = False):
+                 homographyInliersAllPairs: Callable = None, findCameraMatricesManyPairs: Callable = None, trace: Optional[list] = None,
+                 verbose: bool = False):
         self.mImageFeatures = features
         self.n = len(features)
         w, h = image_size
@@ -110,6 +111,7 @@ class SfM:
         self.findHomographyInliers = findHomographyInliers or findHomographyInliers_cv2
         self.homographyInliersAllPairs = homographyInliersAllPairs
         self.findCameraMatricesFromMatch = findCameraMatricesFromMatch or findCameraMatricesFromMatch_cv2
+        self.findCameraMatricesManyPairs = findCameraMatricesManyPairs
         self.findCameraPoseFrom2D3DMatch = findCameraPoseFrom2D3DMatch or findCameraPoseFrom2D3DMatch_cv2
         self.trace = trace
         self.verbose = verbose
@@ -216,11 +218,25 @@ class SfM:
                     self.trace.append({"stage": "homography", "pair": (i, j), "inliers": n_in, "matches": len(m)})
         return sorted(sizes.items(), key=lambda kv: kv[0])
 
+    def _cameraMatricesAhead(self, pairs):
+        """findCameraMatricesFromMatch of every pair in one `findCameraMatricesManyPairs` call (intrinsics, features, pairs, matches)
+        -> [(success, prunedMatches, Pleft, Pright)], or None when the batched function is not given."""
+        if self.findCameraMatricesManyPairs is None:
+            return None
+        return self._timed("essential", self.findCameraMatricesManyPairs, self.mIntrinsics, self.mImageFeatures, pairs,
+                           [self.mFeatureMatchMatrix[l][r] for l, r in pairs])
+
     def findBaselineTriangulation(self):
-        """SfM.cpp:215-321."""
-        for ratio, (i, j) in self.sortViewsForBaseline():
-            ok, pruned, Pl, Pr = self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics,
-                                             self.mFeatureMatchMatrix[i][j], self.mImageFeatures[i], self.mImageFeatures[j])
+        """SfM.cpp:215-321.  With `findCameraMatricesManyPairs`, all candidate pairs are computed in one call before the walk; the
+        walk changes only the match list of the pair at hand, so every stored result is what the call at its turn would return."""
+        order = self.sortViewsForBaseline()
+        ahead = self._cameraMatricesAhead([pr for _, pr in order])
+        for k, (ratio, (i, j)) in enumerate(order):
+            if ahead is not None:
+                ok, pruned, Pl, Pr = ahead[k]
+            else:
+                ok, pruned, Pl, Pr = self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics,
+                                                 self.mFeatureMatchMatrix[i][j], self.mImageFeatures[i], self.mImageFeatures[j])
             if not ok:
                 continue
             if np.float32(len(pruned)) / np.float32(len(self.mFeatureMatchMatrix[i][j])) < POSE_INLIERS_MINIMAL_RATIO:
@@ -363,10 +379,16 @@ class SfM:
                 continue
             self.mCameraPoses[best] = pose
             any_ok = False
-            for good in sorted(self.mGoodViews):
-                l, r = (good, best) if good < best else (best, good)
-                _, pruned, _, _ = self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics, self.mFeatureMatchMatrix[l][r],
-                                              self.mImageFeatures[l], self.mImageFeatures[r])
+            # with `findCameraMatricesManyPairs`, the pairs (good view, new view) in one call up front; each pruned list is stored at
+            # its pair's own turn, since mergeNewPointCloud for an earlier good view reads the lists of later pairs (SfM.cpp:565)
+            lr = [(good, best) if good < best else (best, good) for good in sorted(self.mGoodViews)]
+            ahead = self._cameraMatricesAhead(lr)
+            for k, (l, r) in enumerate(lr):
+                if ahead is not None:
+                    pruned = ahead[k][1]
+                else:
+                    _, pruned, _, _ = self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics, self.mFeatureMatchMatrix[l][r],
+                                                  self.mImageFeatures[l], self.mImageFeatures[r])
                 self.mFeatureMatchMatrix[l][r] = pruned
                 cloud: List[Point3DInMap] = []
                 ok = self._triangulate(l, r, self.mCameraPoses[l], self.mCameraPoses[r], cloud)

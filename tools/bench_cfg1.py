@@ -2,7 +2,8 @@
 hot-path stages on the GPU through the drop-in call shape, beside the same replay on the CPU (cv2 for matching and
 triangulation = the reference's own OpenCV calls, the oracle's Ceres restatement for adjustBundle).  RANSAC stages are
 cv2 in both arms (SURVEY.md 8 f-2); the gpu_batched_essential arm also runs findCameraMatricesFromMatch on the device
-(sfmb200_find_camera_matrices), the gpu_batched_homography arm the homography inliers of all pairs in one device call
+(sfmb200_find_camera_matrices), the gpu_batched_essential_pairs arm the same stage for all pairs of a driver loop in one device
+call (sfmb200_find_camera_matrices_pairs), the gpu_batched_homography arm the homography inliers of all pairs in one device call
 (sfmb200_find_homography_pairs).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
 
     python tools/bench_cfg1.py [--reps 3] [--out gpurun_out/cfg1.json]
@@ -19,7 +20,7 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 
 
-def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, homography=False):
+def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, homography=False, essential_pairs=False):
     from sfm_toy_library_b200 import ransac, runsfm, stages
     kw = {}
     if arm == "gpu":
@@ -30,6 +31,8 @@ def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, ho
             kw["matchAllPairs"] = lambda feats, pairs: stages.matchAllPairs(feats, pairs, ctx=ctx)
         if essential:
             kw["findCameraMatricesFromMatch"] = lambda *a: ransac.findCameraMatricesFromMatch_gpu(*a, ctx=ctx)
+        if essential_pairs:
+            kw["findCameraMatricesManyPairs"] = lambda intr, f, pr, m: ransac.cameraMatricesManyPairs(intr, f, pr, m, ctx=ctx)
         if homography:
             kw["homographyInliersAllPairs"] = lambda f, pr, m: ransac.homographyInliersAllPairs(f, pr, m, ctx=ctx)
     else:
@@ -61,7 +64,10 @@ def measure(reps=3):
     run_arm(cfg1, "gpu", ctx, essential=True)
     runs = [run_arm(cfg1, "gpu", ctx, essential=True) for _ in range(reps)]
     out["gpu_batched_essential"] = min(runs, key=lambda r: r["seconds"]["essential"])
-    out["essential_s"] = {"gpu_batched": out["gpu_batched"]["seconds"]["essential"], "gpu_batched_essential": out["gpu_batched_essential"]["seconds"]["essential"]}
+    run_arm(cfg1, "gpu", ctx, essential_pairs=True)
+    runs = [run_arm(cfg1, "gpu", ctx, essential_pairs=True) for _ in range(reps)]
+    out["gpu_batched_essential_pairs"] = min(runs, key=lambda r: r["seconds"]["essential"])
+    out["essential_s"] = {k: out[k]["seconds"]["essential"] for k in ("gpu_batched", "gpu_batched_essential", "gpu_batched_essential_pairs")}
     run_arm(cfg1, "gpu", ctx, homography=True)
     runs = [run_arm(cfg1, "gpu", ctx, homography=True) for _ in range(reps)]
     out["gpu_batched_homography"] = min(runs, key=lambda r: r["seconds"]["homography"])

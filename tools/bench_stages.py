@@ -152,10 +152,51 @@ def card():
     return torch.cuda.get_device_name(0), pl
 
 
-def measure_essential(ctx, reps=20):
+ESSENTIAL_KERNELS = ("essential_solve_kernel", "essential_score_kernel", "essential_select_kernel", "essential_cheirality_kernel",
+                     "essential_pose_kernel")
+
+
+def synthetic_essential_set(images=50, seed=0):
+    """Seeded all-pairs set: per pair a two-view scene (tests/essential_util.synthetic_scene) of 200-1200 matches at 30-70 %
+    outliers and 0.5 px noise, its points appended to the two images."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from essential_util import synthetic_scene
+    rs = np.random.RandomState(seed)
+    pts = [[] for _ in range(images)]; sizes = [0] * images
+    pairs, mq, mt, off = [], [], [], [0]
+    for i in range(images):
+        for j in range(i + 1, images):
+            n = int(rs.randint(200, 1201)); r = rs.uniform(0.3, 0.7)
+            a, b, *_ = synthetic_scene(int(rs.randint(1 << 30)), n, noise_px=0.5, outliers=r)
+            pts[i].append(a); pts[j].append(b)
+            mq.append(np.arange(n, dtype=np.int32) + sizes[i]); mt.append(np.arange(n, dtype=np.int32) + sizes[j])
+            sizes[i] += n; sizes[j] += n
+            pairs.append((i, j)); off.append(off[-1] + n)
+    return [np.concatenate(p) for p in pts], np.array(pairs, np.int32), np.concatenate(mq), np.concatenate(mt), np.array(off, np.int64)
+
+
+def essential_kernel_ms(fn):
+    """device time per K5 kernel (ms, summed over its launches) of one fn() under torch.profiler"""
+    import torch
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    out = {k: 0.0 for k in ESSENTIAL_KERNELS}
+    for e in prof.events():
+        for k in ESSENTIAL_KERNELS:
+            if k in e.name:
+                out[k] += 1e-3 * e.device_time_total
+    out["total"] = sum(out.values())
+    return out
+
+
+def measure_essential(ctx, reps=20, profile=False):
     """findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) on the 21 crazyhorse pairs of tests/golden/cfg1_crazyhorse.npz:
     sfmb200_find_camera_matrices (host clock around the synchronised call, warmed up, median over reps per pair) against
-    cv2.findEssentialMat(RANSAC, 0.999, 1 px) + cv2.recoverPose on one thread and on all threads."""
+    cv2.findEssentialMat(RANSAC, 0.999, 1 px) + cv2.recoverPose on one thread and on all threads.  Then, in the same run, the 21
+    pairs as 21 single calls and in one sfmb200_find_camera_matrices_pairs call (host clock, median over reps), a seeded synthetic
+    50-image set (1225 pairs) in one call, and with profile=True the per-kernel device time of each from torch.profiler in a
+    separate pass."""
     import cv2
     g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
     K = np.array([[2500, 0, 512], [0, 2500, 384], [0, 0, 1]], np.float32)
@@ -182,12 +223,40 @@ def measure_essential(ctx, reps=20):
         return out
     one = cv_ms(1); allt = cv_ms(os.cpu_count() or 1)
     cv2.setNumThreads(-1)
+
+    feats = [g[f"pts_{i}"] for i in range(len(g["files"]))]
+    ch_pairs = np.array(g["pairs"], np.int32)
+    ch_q = [g[f"match_{p}_q"] for p in range(len(ch_pairs))]; ch_t = [g[f"match_{p}_t"] for p in range(len(ch_pairs))]
+    ch_off = np.zeros(len(ch_pairs) + 1, np.int64); ch_off[1:] = np.cumsum([len(q) for q in ch_q])
+    ch_q = np.concatenate(ch_q); ch_t = np.concatenate(ch_t)
+    sy = synthetic_essential_set()
+
+    def timed(fn, n):
+        fn()
+        ts = []
+        for _ in range(n):
+            t0 = time.perf_counter(); fn(); ts.append(1e3 * (time.perf_counter() - t0))
+        return ts
+    singles = lambda: [ctx.find_camera_matrices(K, a, b) for a, b in pairs]
+    batched = lambda: ctx.find_camera_matrices_pairs(K, feats, ch_pairs, ch_q, ch_t, ch_off)
+    synthetic = lambda: ctx.find_camera_matrices_pairs(K, *sy)
+    t_single, t_batch = [], []
+    for _ in range(reps // 2):                   # alternated, so both see the same state of the shared machine
+        t_single += timed(singles, 1); t_batch += timed(batched, 1)
+    t_syn = timed(synthetic, 5)
+    kernels = {"crazyhorse_21_single_calls": essential_kernel_ms(singles), "crazyhorse_21_one_call": essential_kernel_ms(batched),
+               "synthetic_1225_one_call": essential_kernel_ms(synthetic)} if profile else "not profiled"
     name, pl = card()
     return {"metric": "essential_ransac_pose_ms_per_call", "gpu_median_ms": float(np.median(gpu)), "gpu_max_ms": float(np.max(gpu)),
             "cv2_1thread_median_ms": float(np.median(one)), "cv2_all_threads_median_ms": float(np.median(allt)),
             "speedup_vs_cv2_1thread": float(np.median(one) / np.median(gpu)), "pairs": len(pairs), "matches": [int(len(a)) for a, _ in pairs],
             "card": name, "power_limit": pl, "cpu_threads": os.cpu_count(),
-            "detail": {"gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt}}
+            "crazyhorse_21_single_calls_median_ms": float(np.median(t_single)), "crazyhorse_21_one_call_median_ms": float(np.median(t_batch)),
+            "crazyhorse_21_speedup_one_call": float(np.median(t_single) / np.median(t_batch)),
+            "synthetic_1225_one_call_median_ms": float(np.median(t_syn)), "synthetic_1225_one_call_max_ms": float(np.max(t_syn)),
+            "synthetic_matches": int(sy[4][-1]), "kernel_ms_torch_profiler": kernels,
+            "detail": {"gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt, "crazyhorse_21_single_calls_ms": t_single,
+                       "crazyhorse_21_one_call_ms": t_batch, "synthetic_1225_one_call_ms": t_syn}}
 
 
 def synthetic_homography_set(images=50, seed=0):
@@ -265,7 +334,7 @@ def measure_homography(ctx, images=50, reps=3):
             "kernel_ms_torch_profiler": kernel}
 
 
-def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential")):
+def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential"), profile=False):
     import torch
     from sfm_toy_library_b200 import capi
     own = ctx is None
@@ -279,7 +348,7 @@ def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, st
     if "triangulate" in stages:
         out.append(measure_triangulate(ctx, stream, flush, points, reps))
     if "essential" in stages:
-        out.append(measure_essential(ctx))
+        out.append(measure_essential(ctx, profile=profile))
     if "homography" in stages:
         out.append(measure_homography(ctx, images))
     if own:
@@ -294,8 +363,9 @@ def main():
     ap.add_argument("--points", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography")
+    ap.add_argument("--no-profile", action="store_true", help="skip the torch.profiler kernel split of the essential stage")
     args = ap.parse_args()
-    for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(",")):
+    for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(","), profile=not args.no_profile):
         print(json.dumps(line), flush=True)
 
 
