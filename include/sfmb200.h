@@ -115,6 +115,24 @@ int sfmb200_triangulate_device(sfmb200_ctx* ctx, const float* K, const float* Pl
                                const float* d_pts_left, const float* d_pts_right,
                                const int32_t* d_match_q, const int32_t* d_match_t, int m, float max_reproj_px,
                                float* d_X, uint8_t* d_keep, int32_t* d_n_keep);
+/*
+ * sfmb200_triangulate for every pair of a batch in one call, with the input layout of sfmb200_find_homography_pairs and
+ * sfmb200_find_camera_matrices_pairs (pts / img_off / pairs / match_q / match_t / match_off below), so one set of arrays serves
+ * all three calls.  Pair p's slices of X and keep and n_keep[p] are bitwise what sfmb200_triangulate returns for that pair's
+ * matches and poses, whatever else is in the batch and wherever the pair stands in it.  A pair with no matches gets n_keep 0.
+ *   K [9] float row-major, shared by all pairs; poses [n_pairs * 24]: pair p's Pleft [12] then Pright [12], row-major 3x4 float.
+ *   pts [img_off[n_img] * 2]: key points of all images; img_off [n_img + 1] monotone from 0; pairs [n_pairs * 2] (left, right)
+ *   image; pair p owns matches match_off[p] .. match_off[p+1] (match_q / match_t index the left / right image's key points;
+ *   match_off [n_pairs + 1] monotone from 0).  max_reproj_px as in sfmb200_triangulate.
+ *   X [match_off[n_pairs] * 3], keep [match_off[n_pairs]]; n_keep [n_pairs] survivors per pair, may be NULL.
+ * Inputs are checked on the host before any launch: an image index out of range, non-monotone offsets, match_off[0] != 0 and a
+ * match index outside its image give SFMB200_ERR_INVALID with a message, and the context stays usable.  n_pairs == 0 does
+ * nothing.  One upload, one download and one host synchronisation per call, with one launch of sfmb200_triangulate's kernel per
+ * pair that has matches.
+ */
+int sfmb200_triangulate_pairs(sfmb200_ctx* ctx, const float* K, const float* poses, const float* pts, const int32_t* img_off, int n_img,
+                              const int32_t* pairs, int n_pairs, const int32_t* match_q, const int32_t* match_t, const int64_t* match_off,
+                              float max_reproj_px, float* X, uint8_t* keep, int32_t* n_keep);
 
 /* ---- a-3 / a-4: bundle adjustment ----------------------------------------------------------------------- */
 /* Options = the Ceres options the reference sets (SfMBundleAdjustmentUtils.cpp:171-177) + the Ceres defaults it

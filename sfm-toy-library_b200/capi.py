@@ -182,6 +182,31 @@ class Context:
                                               C.c_float(max_reproj), _p(X, C.c_float), _p(keep, C.c_uint8), C.byref(nk)))
         return X[:m], keep[:m], nk.value
 
+    def triangulate_pairs(self, K, poses, points, pairs, match_q, match_t, match_off, max_reproj=MIN_REPROJECTION_ERROR):
+        """sfmb200_triangulate_pairs: triangulate for every pair in one call, with the arguments of find_camera_matrices_pairs
+        (points: list of [n_i, 2] key points per image; pairs [P, 2]; match_q / match_t: all pairs' matches concatenated, pair p
+        owning match_off[p]:match_off[p+1]).  poses [P, 2, 3, 4]: pair p's (Pleft, Pright).
+        Returns (X [sum of matches, 3], keep [sum of matches], n_keep [P])."""
+        K = np.ascontiguousarray(K, np.float32).reshape(9)
+        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
+        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
+        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
+        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
+        moff = np.ascontiguousarray(match_off, np.int64)
+        P = pairs.shape[0]
+        poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 24)
+        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
+            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+        if poses.shape[0] != P:
+            raise ValueError("poses must hold one (Pleft, Pright) per pair")
+        M = mq.shape[0]
+        X = np.empty((max(M, 1), 3), np.float32); keep = np.empty(max(M, 1), np.uint8); nk = np.zeros(max(P, 1), np.int32)
+        self._check(lib().sfmb200_triangulate_pairs(self._h, _p(K, C.c_float), _p(poses, C.c_float), _p(allp, C.c_float), _p(img_off, C.c_int32),
+                                                    len(pts), _p(pairs, C.c_int32), P, _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64),
+                                                    C.c_float(max_reproj), _p(X, C.c_float), _p(keep, C.c_uint8), _p(nk, C.c_int32)))
+        return X[:M], keep[:M], nk[:P]
+
     def triangulate_device(self, K, Pl, Pr, d_left, d_right, d_mq, d_mt, m, d_X, d_keep, d_nkeep, max_reproj=MIN_REPROJECTION_ERROR):
         """All d_* are raw device pointers (ints); nothing is synchronised."""
         K = np.ascontiguousarray(K, np.float32).reshape(9); Pl = np.ascontiguousarray(Pl, np.float32).reshape(12)

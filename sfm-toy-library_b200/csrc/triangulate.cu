@@ -10,6 +10,9 @@
 // (Hestenes) Jacobi in double -- the algorithm cv::SVD uses -- float dehomogenisation with a float reciprocal,
 // double projection with the float-rvec round-tripped rotation, float pixel error, keep flag.
 // HBM traffic: 16 B in (+8 B indices) and 13 B out per match; everything else lives in registers.
+// sfmb200_triangulate_pairs runs the same kernel for many pairs: one upload of all key points and matches, one launch per pair
+// with that pair's parameters and slices, one download.  It does not use a kernel of its own: ptxas decides per kernel which
+// multiplies and adds it contracts into FMAs, so a second kernel with the same source rounds differently on some matches.
 #include "common.cuh"
 #include "dlt_math.cuh"
 #include <cfloat>
@@ -180,6 +183,81 @@ int sfmb200_triangulate(sfmb200_ctx* ctx, const float* K, const float* Pl, const
     SFM_CUDA(ctx, cudaMemcpyAsync(&hn, d_n, 4, cudaMemcpyDeviceToHost, ctx->stream));
     SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (n_keep) *n_keep = hn;
+    return SFMB200_OK;
+}
+
+int sfmb200_triangulate_pairs(sfmb200_ctx* ctx, const float* K, const float* poses, const float* pts, const int32_t* img_off, int n_img,
+                              const int32_t* pairs, int n_pairs, const int32_t* match_q, const int32_t* match_t, const int64_t* match_off,
+                              float max_reproj_px, float* X, uint8_t* keep, int32_t* n_keep) {
+    if (!ctx || n_img < 0 || n_pairs < 0) return SFMB200_ERR_INVALID;
+    if (n_pairs == 0) return SFMB200_OK;
+    if (!K || !poses || !img_off || !pairs || !match_off) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    if (img_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off[0] must be 0");
+    for (int i = 0; i < n_img; ++i)
+        if (img_off[i + 1] < img_off[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off is not monotone at image %d", i);
+    if (img_off[n_img] > 0 && !pts) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    if (match_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off[0] must be 0");
+    for (int p = 0; p < n_pairs; ++p) {
+        if (match_off[p + 1] < match_off[p]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off is not monotone at pair %d", p);
+        if (pairs[2 * p] < 0 || pairs[2 * p] >= n_img || pairs[2 * p + 1] < 0 || pairs[2 * p + 1] >= n_img)
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "pair %d names an image outside [0, %d)", p, n_img);
+    }
+    const int64_t M = match_off[n_pairs];
+    if (M > INT32_MAX) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "too many matches in one call");
+    if (M > 0 && (!match_q || !match_t || !X || !keep)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    for (int p = 0; p < n_pairs; ++p) {
+        const int nl = img_off[pairs[2 * p] + 1] - img_off[pairs[2 * p]], nr = img_off[pairs[2 * p + 1] + 1] - img_off[pairs[2 * p + 1]];
+        for (int64_t k = match_off[p]; k < match_off[p + 1]; ++k)
+            if (match_q[k] < 0 || match_q[k] >= nl || match_t[k] < 0 || match_t[k] >= nr)
+                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %lld of pair %d indexes outside its images' key points", (long long)k, p);
+    }
+    if (n_keep) memset(n_keep, 0, sizeof(int32_t) * (size_t)n_pairs);
+    if (M == 0) return SFMB200_OK;
+    const int64_t NP = img_off[n_img];
+
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    SFM_CUDA(ctx, cudaSetDevice(ctx->device));
+    // pinned staging and device scratch share one layout: key points | match_q | match_t | n_keep | X | keep.  The upload runs up to
+    // n_keep (zeroed here), the download from n_keep on.
+    const size_t bytes = Carver::pad(8 * (size_t)NP) + 2 * Carver::pad(4 * (size_t)M) + Carver::pad(4 * (size_t)n_pairs) +
+                         Carver::pad(12 * (size_t)M) + Carver::pad((size_t)M) + 256;
+    SFM_CUDA(ctx, ctx->pinned.reserve(bytes));
+    SFM_CUDA(ctx, ctx->scratch.reserve(bytes));
+    Carver hc(ctx->pinned.p);
+    float* h_pts = hc.take<float>(2 * (size_t)NP);
+    int32_t* h_mq = hc.take<int32_t>((size_t)M);
+    int32_t* h_mt = hc.take<int32_t>((size_t)M);
+    int32_t* h_nk = hc.take<int32_t>(n_pairs);
+    float* h_X = hc.take<float>(3 * (size_t)M);
+    uint8_t* h_keep = hc.take<uint8_t>((size_t)M);
+    const size_t up_len = (char*)(h_nk + n_pairs) - (char*)ctx->pinned.p;
+    const size_t down_off = (char*)h_nk - (char*)ctx->pinned.p, down_len = hc.off - down_off;
+    if (NP > 0) memcpy(h_pts, pts, 8 * (size_t)NP);
+    memcpy(h_mq, match_q, 4 * (size_t)M);
+    memcpy(h_mt, match_t, 4 * (size_t)M);
+    memset(h_nk, 0, 4 * (size_t)n_pairs);
+    Carver cv(ctx->scratch.p);
+    const float2* d_pts = (const float2*)cv.take<float>(2 * (size_t)NP);
+    const int32_t* d_mq = cv.take<int32_t>((size_t)M);
+    const int32_t* d_mt = cv.take<int32_t>((size_t)M);
+    int32_t* d_nk = cv.take<int32_t>(n_pairs);
+    float* d_X = cv.take<float>(3 * (size_t)M);
+    uint8_t* d_keep = cv.take<uint8_t>((size_t)M);
+    SFM_CUDA(ctx, cudaMemcpyAsync(ctx->scratch.p, ctx->pinned.p, up_len, cudaMemcpyHostToDevice, ctx->stream));
+    for (int p = 0; p < n_pairs; ++p) {
+        const int64_t off = match_off[p];
+        const int m = (int)(match_off[p + 1] - off);
+        if (m == 0) continue;
+        TriParams P; make_params(K, poses + 24 * (size_t)p, poses + 24 * (size_t)p + 12, max_reproj_px, P);
+        triangulate_kernel<<<ceil_div(m, 128), 128, 0, ctx->stream>>>(P, d_pts + img_off[pairs[2 * p]], d_pts + img_off[pairs[2 * p + 1]],
+                                                                      d_mq + off, d_mt + off, m, d_X + 3 * off, d_keep + off, d_nk + p);
+        SFM_LAUNCH_CHECK(ctx);
+    }
+    SFM_CUDA(ctx, cudaMemcpyAsync((char*)ctx->pinned.p + down_off, (char*)ctx->scratch.p + down_off, down_len, cudaMemcpyDeviceToHost, ctx->stream));
+    SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    memcpy(X, h_X, 12 * (size_t)M);
+    memcpy(keep, h_keep, (size_t)M);
+    if (n_keep) memcpy(n_keep, h_nk, 4 * (size_t)n_pairs);
     return SFMB200_OK;
 }
 

@@ -93,8 +93,8 @@ class SfM:
     def __init__(self, features: List[Features], image_size, *, matchFeatures: Callable = None, triangulateViews: Callable = None,
                  adjustBundle: Callable = None, matchAllPairs: Callable = None, findHomographyInliers: Callable = None,
                  findCameraMatricesFromMatch: Callable = None, findCameraPoseFrom2D3DMatch: Callable = None,
-                 homographyInliersAllPairs: Callable = None, findCameraMatricesManyPairs: Callable = None, trace: Optional[list] = None,
-                 verbose: bool = False):
+                 homographyInliersAllPairs: Callable = None, findCameraMatricesManyPairs: Callable = None,
+                 triangulateManyPairs: Callable = None, trace: Optional[list] = None, verbose: bool = False):
         self.mImageFeatures = features
         self.n = len(features)
         w, h = image_size
@@ -112,6 +112,7 @@ class SfM:
         self.homographyInliersAllPairs = homographyInliersAllPairs
         self.findCameraMatricesFromMatch = findCameraMatricesFromMatch or findCameraMatricesFromMatch_cv2
         self.findCameraMatricesManyPairs = findCameraMatricesManyPairs
+        self.triangulateManyPairs = triangulateManyPairs
         self.findCameraPoseFrom2D3DMatch = findCameraPoseFrom2D3DMatch or findCameraPoseFrom2D3DMatch_cv2
         self.trace = trace
         self.verbose = verbose
@@ -256,12 +257,15 @@ class SfM:
         n0 = len(cloud)
         ok = self._timed("triangulate", self.triangulateViews, self.mIntrinsics, ImagePair(i, j), self.mFeatureMatchMatrix[i][j],
                          self.mImageFeatures[i], self.mImageFeatures[j], Pl, Pr, cloud)
+        self._traceTriangulation(i, j, Pl, Pr, cloud[n0:])
+        return ok
+
+    def _traceTriangulation(self, i, j, Pl, Pr, new_points):
         if self.trace is not None:
             self.trace.append({"stage": "triangulate", "pair": (i, j), "K": self.mIntrinsics.K.copy(), "Pl": np.array(Pl, np.float32),
                                "Pr": np.array(Pr, np.float32), "matches": self.mFeatureMatchMatrix[i][j].copy(),
-                               "X": np.array([p.p for p in cloud[n0:]], np.float32).reshape(-1, 3),
-                               "back": np.array([[p.originatingViews[i], p.originatingViews[j]] for p in cloud[n0:]], np.int32).reshape(-1, 2)})
-        return ok
+                               "X": np.array([p.p for p in new_points], np.float32).reshape(-1, 3),
+                               "back": np.array([[p.originatingViews[i], p.originatingViews[j]] for p in new_points], np.int32).reshape(-1, 2)})
 
     def adjustCurrentBundle(self):
         """SfM.cpp:324-330."""
@@ -383,6 +387,16 @@ class SfM:
             # its pair's own turn, since mergeNewPointCloud for an earlier good view reads the lists of later pairs (SfM.cpp:565)
             lr = [(good, best) if good < best else (best, good) for good in sorted(self.mGoodViews)]
             ahead = self._cameraMatricesAhead(lr)
+            # with `triangulateManyPairs` (intrinsics, features, pairs, matches, poses) -> one cloud per pair, every pair is
+            # triangulated in one call up front: the poses and K do not change inside this loop and mergeNewPointCloud does not
+            # write match lists, so each cloud is what the call at its pair's turn would return
+            clouds = None
+            if self.triangulateManyPairs is not None:
+                if ahead is None:
+                    ahead = [self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics, self.mFeatureMatchMatrix[l][r],
+                                         self.mImageFeatures[l], self.mImageFeatures[r]) for l, r in lr]
+                clouds = self._timed("triangulate", self.triangulateManyPairs, self.mIntrinsics, self.mImageFeatures, lr, [a[1] for a in ahead],
+                                     [(self.mCameraPoses[l], self.mCameraPoses[r]) for l, r in lr])
             for k, (l, r) in enumerate(lr):
                 if ahead is not None:
                     pruned = ahead[k][1]
@@ -390,8 +404,12 @@ class SfM:
                     _, pruned, _, _ = self._timed("essential", self.findCameraMatricesFromMatch, self.mIntrinsics, self.mFeatureMatchMatrix[l][r],
                                                   self.mImageFeatures[l], self.mImageFeatures[r])
                 self.mFeatureMatchMatrix[l][r] = pruned
-                cloud: List[Point3DInMap] = []
-                ok = self._triangulate(l, r, self.mCameraPoses[l], self.mCameraPoses[r], cloud)
+                if clouds is None:
+                    cloud: List[Point3DInMap] = []
+                    ok = self._triangulate(l, r, self.mCameraPoses[l], self.mCameraPoses[r], cloud)
+                else:
+                    cloud, ok = clouds[k], True
+                    self._traceTriangulation(l, r, self.mCameraPoses[l], self.mCameraPoses[r], cloud)
                 if ok:
                     nn, nm = self.mergeNewPointCloud(cloud)
                     if self.verbose:

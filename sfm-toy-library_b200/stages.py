@@ -137,6 +137,24 @@ def triangulateViews(intrinsics: Intrinsics, imagePair: ImagePair, matches: np.n
     return True
 
 
+def triangulateManyPairs(intrinsics: Intrinsics, features: List[Features], pairs, matches, poses, ctx=None) -> List[PointCloud]:
+    """triangulateViews for every pair in one device call (sfmb200_triangulate_pairs).  features: per image Features; pairs
+    [(i, j), ...]; matches: per pair a structured array with queryIdx / trainIdx; poses: per pair (Pleft, Pright).  Returns one
+    PointCloud per pair, each exactly what triangulateViews appends for that pair."""
+    ctx = ctx or default_context()
+    if len(pairs) == 0:
+        return []
+    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
+    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
+    X, keep, _ = ctx.triangulate_pairs(intrinsics.K, [np.stack([Pl, Pr]) for Pl, Pr in poses], [f.points for f in features], pairs, mq, mt, off,
+                                       capi.MIN_REPROJECTION_ERROR)
+    clouds = []
+    for p, (left, right) in enumerate(pairs):
+        clouds.append([Point3DInMap(X[i].copy(), {int(left): int(mq[i]), int(right): int(mt[i])})
+                       for i in off[p] + np.nonzero(keep[off[p]:off[p + 1]])[0]])
+    return clouds
+
+
 def pose_is_empty(pose) -> bool:
     """The reference's "empty pose" rule (SfMBundleAdjustmentUtils.cpp:118-122, :196-199): R diagonal exactly zero."""
     pose = np.asarray(pose, np.float32).reshape(3, 4)

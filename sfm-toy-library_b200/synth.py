@@ -167,3 +167,25 @@ def make_triangulation_problem(m=1_000_000, seed=0, noise=1e-3, outlier_frac=0.0
         idx = rs.choice(m, nb, replace=False)
         out[1][idx] += rs.uniform(-60, 60, (nb, 2)).astype(np.float32)
     return dict(K=TEST_K.copy(), Pl=Pl, Pr=Pr, ptsL=out[0], ptsR=out[1], X_true=X.astype(np.float32))
+
+
+def make_triangulation_pairs(images=50, seed=0):
+    """All i < j pairs of `images` views in the layout of sfmb200_triangulate_pairs: pair k is make_triangulation_problem(m, seed
+    = 100000 * seed + k) with 400-1200 matches, its two views swapped for odd k, so the pairs alternate between two sets of poses.
+    Each pair's key points are appended to its two images.
+    Returns (K, poses [P, 2, 3, 4], points per image, pairs [P, 2], match_q, match_t, match_off [P + 1])."""
+    rs = np.random.RandomState(seed)
+    pts = [[] for _ in range(images)]; sizes = [0] * images
+    pairs, poses, mq, mt, off = [], [], [], [], [0]
+    for i in range(images):
+        for j in range(i + 1, images):
+            k = len(pairs); m = int(rs.randint(400, 1201))
+            pr = make_triangulation_problem(m, seed=100000 * seed + k)
+            (Pl, a), (Pr, b) = ((pr["Pl"], pr["ptsL"]), (pr["Pr"], pr["ptsR"]))[::1 if k % 2 == 0 else -1]
+            pts[i].append(a); pts[j].append(b)
+            mq.append(np.arange(m, dtype=np.int32) + sizes[i]); mt.append(np.arange(m, dtype=np.int32) + sizes[j])
+            sizes[i] += m; sizes[j] += m
+            pairs.append((i, j)); poses.append((Pl, Pr)); off.append(off[-1] + m)
+    return (TEST_K.copy(), np.array(poses, np.float32), [np.concatenate(p) if p else np.zeros((0, 2), np.float32) for p in pts],
+            np.array(pairs, np.int32).reshape(-1, 2), np.concatenate(mq) if mq else np.zeros(0, np.int32),
+            np.concatenate(mt) if mt else np.zeros(0, np.int32), np.array(off, np.int64))

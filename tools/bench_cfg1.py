@@ -4,7 +4,9 @@ triangulation = the reference's own OpenCV calls, the oracle's Ceres restatement
 cv2 in both arms (SURVEY.md 8 f-2); the gpu_batched_essential arm also runs findCameraMatricesFromMatch on the device
 (sfmb200_find_camera_matrices), the gpu_batched_essential_pairs arm the same stage for all pairs of a driver loop in one device
 call (sfmb200_find_camera_matrices_pairs), the gpu_batched_homography arm the homography inliers of all pairs in one device call
-(sfmb200_find_homography_pairs).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
+(sfmb200_find_homography_pairs).  The triangulate_s line compares, alternated in the same run, the gpu_batched_essential_pairs
+driver (one triangulateViews call per pair) with the gpu_batched_triangulate_pairs driver, which also triangulates all pairs of
+an added view in one device call (sfmb200_triangulate_pairs).  Input: tests/golden/cfg1_crazyhorse.npz (pre-extracted ORB features).
 
     python tools/bench_cfg1.py [--reps 3] [--out gpurun_out/cfg1.json]
 """
@@ -15,12 +17,13 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests")); sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 
 
-def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, homography=False, essential_pairs=False):
+def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, homography=False, essential_pairs=False,
+            triangulate_pairs=False):
     from sfm_toy_library_b200 import ransac, runsfm, stages
     kw = {}
     if arm == "gpu":
@@ -33,6 +36,8 @@ def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, ho
             kw["findCameraMatricesFromMatch"] = lambda *a: ransac.findCameraMatricesFromMatch_gpu(*a, ctx=ctx)
         if essential_pairs:
             kw["findCameraMatricesManyPairs"] = lambda intr, f, pr, m: ransac.cameraMatricesManyPairs(intr, f, pr, m, ctx=ctx)
+        if triangulate_pairs:
+            kw["triangulateManyPairs"] = lambda *a: stages.triangulateManyPairs(*a, ctx=ctx)
         if homography:
             kw["homographyInliersAllPairs"] = lambda f, pr, m: ransac.homographyInliersAllPairs(f, pr, m, ctx=ctx)
     else:
@@ -49,6 +54,23 @@ def run_arm(cfg1, arm, ctx=None, batched=True, threads=None, essential=False, ho
     wall = time.perf_counter() - t0
     return {"wall_s": wall, "seconds": dict(sfm.seconds), "calls": dict(sfm.calls), "cloud": len(sfm.mReconstructionCloud),
             "hot_path_s": sfm.seconds["match"] + sfm.seconds["triangulate"] + sfm.seconds["bundle"]}
+
+
+def measure_triangulate(cfg1, ctx, reps=3):
+    """seconds["triangulate"] of the driver with the batched essential stage, triangulating pair by pair against one
+    triangulateManyPairs call per added view; the two drivers alternate, the best of reps of each is kept"""
+    from bench_stages import card
+    arms = {"gpu_batched_essential_pairs": dict(essential_pairs=True), "gpu_batched_triangulate_pairs": dict(essential_pairs=True, triangulate_pairs=True)}
+    runs = {k: [] for k in arms}
+    for kw in arms.values():
+        run_arm(cfg1, "gpu", ctx, **kw)
+    for _ in range(reps):
+        for k, kw in arms.items():
+            runs[k].append(run_arm(cfg1, "gpu", ctx, **kw))
+    best = {k: min(r, key=lambda x: x["seconds"]["triangulate"]) for k, r in runs.items()}
+    name, pl = card()
+    return {"card": name, "power_limit": pl, **{k: {"seconds": b["seconds"]["triangulate"], "calls": b["calls"]["triangulate"],
+                                                    "all_runs_s": [x["seconds"]["triangulate"] for x in runs[k]]} for k, b in best.items()}}
 
 
 def measure(reps=3):
@@ -68,6 +90,7 @@ def measure(reps=3):
     runs = [run_arm(cfg1, "gpu", ctx, essential_pairs=True) for _ in range(reps)]
     out["gpu_batched_essential_pairs"] = min(runs, key=lambda r: r["seconds"]["essential"])
     out["essential_s"] = {k: out[k]["seconds"]["essential"] for k in ("gpu_batched", "gpu_batched_essential", "gpu_batched_essential_pairs")}
+    out["triangulate_s"] = measure_triangulate(cfg1, ctx, reps)
     run_arm(cfg1, "gpu", ctx, homography=True)
     runs = [run_arm(cfg1, "gpu", ctx, homography=True) for _ in range(reps)]
     out["gpu_batched_homography"] = min(runs, key=lambda r: r["seconds"]["homography"])

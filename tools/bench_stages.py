@@ -334,6 +334,70 @@ def measure_homography(ctx, images=50, reps=3):
             "kernel_ms_torch_profiler": kernel}
 
 
+def measure_triangulate_pairs(ctx, reps=20, profile=False):
+    """triangulateViews (SfMStereoUtilities.cpp:120-206) batched per driver loop: host clock around the synchronised call, warmed up,
+    median and max over reps, the two arms alternated in the same run.
+      - the 20 addMoreViewsToReconstruction triangulations of tests/golden/cfg1_crazyhorse.npz (every recorded call after the
+        baseline's): 20 sfmb200_triangulate calls against one sfmb200_triangulate_pairs call per added view (5 calls);
+      - synth.make_triangulation_pairs(50): 1225 single calls against one call.
+    With profile=True, the device time of triangulate_kernel / triangulate_pairs_kernel of each arm from torch.profiler in a
+    separate pass."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from cfg1_util import Cfg1
+    from sfm_toy_library_b200 import synth
+    cfg1 = Cfg1()
+    pts = [f.points for f in cfg1.features]
+    loops = {}
+    for k in range(1, cfg1.n_tri):
+        loops.setdefault(cfg1.tri(k)["K"].tobytes(), []).append(cfg1.tri(k))
+    loops = list(loops.values())
+    ch_single = [(c["K"], c["Pl"], c["Pr"], pts[int(c["pair"][0])], pts[int(c["pair"][1])], c["mq"], c["mt"]) for lp in loops for c in lp]
+    ch_batch = []
+    for lp in loops:
+        off = np.zeros(len(lp) + 1, np.int64); off[1:] = np.cumsum([len(c["mq"]) for c in lp])
+        ch_batch.append((lp[0]["K"], [(c["Pl"], c["Pr"]) for c in lp], pts, [tuple(int(x) for x in c["pair"]) for c in lp],
+                         np.concatenate([c["mq"] for c in lp]), np.concatenate([c["mt"] for c in lp]), off))
+    K, poses, spts, spairs, smq, smt, soff = sy = synth.make_triangulation_pairs(50, seed=0)
+    sy_single = [(K, poses[p][0], poses[p][1], spts[i], spts[j], smq[soff[p]:soff[p + 1]], smt[soff[p]:soff[p + 1]]) for p, (i, j) in enumerate(spairs)]
+    arms = {"crazyhorse_20_single_calls": lambda: [ctx.triangulate(*a) for a in ch_single],
+            "crazyhorse_20_in_5_calls": lambda: [ctx.triangulate_pairs(*a) for a in ch_batch],
+            "synthetic_1225_single_calls": lambda: [ctx.triangulate(*a) for a in sy_single],
+            "synthetic_1225_one_call": lambda: ctx.triangulate_pairs(*sy)}
+    per_call = []                                       # one single call at a time, per crazyhorse call
+    for a in ch_single:
+        ctx.triangulate(*a)
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter(); ctx.triangulate(*a); ts.append(1e3 * (time.perf_counter() - t0))
+        per_call.append(float(np.median(ts)))
+    times = {k: [] for k in arms}
+    for f in arms.values():
+        f()
+    for _ in range(reps):                               # alternated, so both arms see the same state of the shared machine
+        for k, f in arms.items():
+            t0 = time.perf_counter(); f(); times[k].append(1e3 * (time.perf_counter() - t0))
+    kernels = "not profiled"
+    if profile:
+        import torch
+        kernels = {}
+        for k, f in arms.items():
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                f()
+                torch.cuda.synchronize()
+            ev = [e for e in prof.events() if "triangulate" in e.name and "kernel" in e.name]
+            kernels[k] = {"ms": 1e-3 * sum(e.device_time_total for e in ev), "launches": len(ev)}
+    name, pl = card()
+    out = {"metric": "triangulate_pairs_ms", "card": name, "power_limit": pl, "reps": reps,
+           "crazyhorse_matches_per_call": [int(len(a[5])) for a in ch_single], "crazyhorse_calls_per_added_view": [len(lp) for lp in loops],
+           "crazyhorse_single_call_median_ms": float(np.median(per_call)), "crazyhorse_single_call_max_ms": float(np.max(per_call)),
+           "synthetic_pairs": len(spairs), "synthetic_matches": int(soff[-1]), "kernel_ms_torch_profiler": kernels}
+    for k, ts in times.items():
+        out[k + "_median_ms"] = float(np.median(ts)); out[k + "_max_ms"] = float(np.max(ts))
+    out["crazyhorse_speedup_batched"] = out["crazyhorse_20_single_calls_median_ms"] / out["crazyhorse_20_in_5_calls_median_ms"]
+    out["synthetic_speedup_batched"] = out["synthetic_1225_single_calls_median_ms"] / out["synthetic_1225_one_call_median_ms"]
+    return out
+
+
 def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential"), profile=False):
     import torch
     from sfm_toy_library_b200 import capi
@@ -351,6 +415,8 @@ def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, st
         out.append(measure_essential(ctx, profile=profile))
     if "homography" in stages:
         out.append(measure_homography(ctx, images))
+    if "triangulate-pairs" in stages:
+        out.append(measure_triangulate_pairs(ctx, profile=profile))
     if own:
         ctx.close()
     return out
@@ -362,8 +428,8 @@ def main():
     ap.add_argument("--features", type=int, default=5000)
     ap.add_argument("--points", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography")
-    ap.add_argument("--no-profile", action="store_true", help="skip the torch.profiler kernel split of the essential stage")
+    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography, triangulate-pairs")
+    ap.add_argument("--no-profile", action="store_true", help="skip the torch.profiler kernel split of the essential and triangulate-pairs stages")
     args = ap.parse_args()
     for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(","), profile=not args.no_profile):
         print(json.dumps(line), flush=True)
