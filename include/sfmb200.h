@@ -95,6 +95,25 @@ int sfmb200_match_pairs(sfmb200_ctx* ctx, const sfmb200_descset* set, const int3
 int sfmb200_match_pairs_device(sfmb200_ctx* ctx, const sfmb200_descset* set, const int32_t* pairs, int n_pairs, double ratio,
                                int32_t* d_out_q, int32_t* d_out_t, float* d_out_d, int32_t* d_pair_start, int64_t* d_total);
 
+/* ---- image-pair batches: the input layout of the *_pairs calls ------------------------------------------------ */
+/*
+ * sfmb200_triangulate_pairs, sfmb200_find_camera_matrices_pairs and sfmb200_find_homography_pairs run a stage for many image pairs
+ * in one call.  They take the same arrays, so one set of arrays serves all three:
+ *   pts [img_off[n_img] * 2]   float pixel coordinates of the key points of all images; image i owns pts[2 img_off[i] .. 2 img_off[i+1])
+ *   img_off [n_img + 1]        img_off[0] = 0, monotone
+ *   pairs [n_pairs * 2]        (left image, right image), each in [0, n_img)
+ *   match_q / match_t          per match, the key point index in the left / right image of its pair; pair p owns matches
+ *                              match_off[p] .. match_off[p+1]
+ *   match_off [n_pairs + 1]    match_off[0] = 0, monotone; M = match_off[n_pairs] matches in all
+ * The arrays are checked on the host before any launch.  Each of the following gives SFMB200_ERR_INVALID with a message, and the
+ * context stays usable: a needed array is NULL; img_off[0] != 0 or img_off not monotone; match_off[0] != 0 or match_off not
+ * monotone; a pair names an image outside [0, n_img); M is above the call's limit; a match indexes outside its image's key points.
+ * Where the three calls differ:
+ *   - the limit on M: INT32_MAX for sfmb200_triangulate_pairs, INT32_MAX / 2 for the other two;
+ *   - n_pairs == 0: sfmb200_triangulate_pairs and sfmb200_find_camera_matrices_pairs return SFMB200_OK without reading the arrays
+ *     (after their option and K checks, where they have them); sfmb200_find_homography_pairs still checks img_off and pts.
+ */
+
 /* ---- a-2 (+ a-6): two-view triangulation ---------------------------------------------------------------- */
 /*
  * triangulateViews (SfMStereoUtilities.cpp:120-206) on flat arrays:
@@ -116,19 +135,15 @@ int sfmb200_triangulate_device(sfmb200_ctx* ctx, const float* K, const float* Pl
                                const int32_t* d_match_q, const int32_t* d_match_t, int m, float max_reproj_px,
                                float* d_X, uint8_t* d_keep, int32_t* d_n_keep);
 /*
- * sfmb200_triangulate for every pair of a batch in one call, with the input layout of sfmb200_find_homography_pairs and
- * sfmb200_find_camera_matrices_pairs (pts / img_off / pairs / match_q / match_t / match_off below), so one set of arrays serves
- * all three calls.  Pair p's slices of X and keep and n_keep[p] are bitwise what sfmb200_triangulate returns for that pair's
- * matches and poses, whatever else is in the batch and wherever the pair stands in it.  A pair with no matches gets n_keep 0.
+ * sfmb200_triangulate for every pair of an image-pair batch in one call; pts / img_off / pairs / match_q / match_t / match_off,
+ * their checks and n_pairs == 0 are described under "image-pair batches" above.  Pair p's slices of X and keep and n_keep[p] are
+ * bitwise what sfmb200_triangulate returns for that pair's matches and poses, whatever else is in the batch and wherever the pair
+ * stands in it.  A pair with no matches gets n_keep 0.
  *   K [9] float row-major, shared by all pairs; poses [n_pairs * 24]: pair p's Pleft [12] then Pright [12], row-major 3x4 float.
- *   pts [img_off[n_img] * 2]: key points of all images; img_off [n_img + 1] monotone from 0; pairs [n_pairs * 2] (left, right)
- *   image; pair p owns matches match_off[p] .. match_off[p+1] (match_q / match_t index the left / right image's key points;
- *   match_off [n_pairs + 1] monotone from 0).  max_reproj_px as in sfmb200_triangulate.
+ *   max_reproj_px as in sfmb200_triangulate.
  *   X [match_off[n_pairs] * 3], keep [match_off[n_pairs]]; n_keep [n_pairs] survivors per pair, may be NULL.
- * Inputs are checked on the host before any launch: an image index out of range, non-monotone offsets, match_off[0] != 0 and a
- * match index outside its image give SFMB200_ERR_INVALID with a message, and the context stays usable.  n_pairs == 0 does
- * nothing.  One upload, one download and one host synchronisation per call, with one launch of sfmb200_triangulate's kernel per
- * pair that has matches.
+ * One upload, one download and one host synchronisation per call, with one launch of sfmb200_triangulate's kernel per pair that
+ * has matches.
  */
 int sfmb200_triangulate_pairs(sfmb200_ctx* ctx, const float* K, const float* poses, const float* pts, const int32_t* img_off, int n_img,
                               const int32_t* pairs, int n_pairs, const int32_t* match_q, const int32_t* match_t, const int64_t* match_off,
@@ -300,20 +315,17 @@ int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* 
 int sfmb200_five_point(sfmb200_ctx* ctx, const double* x1, const double* x2, int ns, double* E, int32_t* nsol);
 int sfmb200_essential_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, int32_t* nsol, int32_t* counts);
 /*
- * sfmb200_find_camera_matrices for every pair of a batch in one call, with the input layout of sfmb200_find_homography_pairs
- * (pts / img_off / pairs / match_q / match_t / match_off below), so one set of arrays serves both calls.  Pair p's outputs
+ * sfmb200_find_camera_matrices for every pair of an image-pair batch in one call; pts / img_off / pairs / match_q / match_t /
+ * match_off, their checks and n_pairs == 0 are described under "image-pair batches" above.  Pair p's outputs
  * (E, R, t, its slices of both masks, summary[p]) are bitwise what sfmb200_find_camera_matrices returns for that pair's matches
  * with the same options, whatever else is in the batch and wherever the pair stands in it: one seed covers the call and every
  * pair draws its samples from it as a single call does.  Per pair as in the single call: m < 5 gives found = 0 and zeros, m == 5
  * one sample, no model found = 0 with zeros.
- *   K [9] float row-major, shared by all pairs.  pts [img_off[n_img] * 2]: key points of all images; img_off [n_img + 1]
- *   monotone from 0; pairs [n_pairs * 2] (left, right) image; pair p owns matches match_off[p] .. match_off[p+1] (match_q /
- *   match_t index the left / right image's key points; match_off [n_pairs + 1] monotone from 0).
+ *   K [9] float row-major, shared by all pairs.
  *   E [n_pairs * 9], R [n_pairs * 9], t [n_pairs * 3]: any may be NULL.  inlier_mask / pose_mask [match_off[n_pairs]]: either
  *   may be NULL.  summary [n_pairs]: may be NULL.  opt NULL = defaults.
- * Inputs are checked on the host before any launch: an image index out of range, non-monotone offsets, match_off[0] != 0, a match
- * index outside its image and the option / K checks of the single call give SFMB200_ERR_INVALID with a message, and the context
- * stays usable.  n_pairs == 0 does nothing.  One upload, one download, one host synchronisation per call.  The pairs run in
+ * The option and K checks of the single call come before the batch's.  One upload, one download, one host synchronisation per
+ * call.  The pairs run in
  * consecutive groups whose hypotheses (10 x 96 B per sample, 0.96 MB per pair at max_iters 1000) fit 256 MB of device memory,
  * enqueued back to back.
  */
@@ -339,10 +351,9 @@ int sfmb200_find_camera_matrices_pairs(sfmb200_ctx* ctx, const float* K, const f
  * threshold could in principle flip; on those pairs the closest point is 1e-3 threshold^2 away.
  * n == 4 follows findHomography: the DLT of the four points, no checks, no refinement, mask all ones.  n < 4 or no model: found = 0,
  * n_inliers = 0, H and mask zero (the reference's `homography.empty()` branch).
- *   pts [img_off[n_img] * 2]   key points of all images; image i owns pts[2 img_off[i] .. 2 img_off[i+1]); img_off [n_img + 1] monotone
- *   pairs [n_pairs * 2]        (left image, right image)
- *   match_q / match_t          per match, the key point index in the left / right image; pair p owns matches match_off[p] ..
- *                              match_off[p+1]; match_off [n_pairs + 1], match_off[0] = 0, monotone
+ *   pts / img_off / pairs / match_q / match_t / match_off: an image-pair batch; the layout, its checks and n_pairs == 0 are
+ *   described under "image-pair batches" above.  The option checks come first, and record_trace = 1 refuses n_pairs * max_iters
+ *   above INT32_MAX / 4.
  *   H [n_pairs * 9]            row-major, h22 = 1; may be NULL.  mask [match_off[n_pairs]]: may be NULL.  summary [n_pairs]: may be NULL.
  * One CTA per pair, one host synchronisation per call.  Same inputs: bitwise-identical outputs, whether a pair is alone in a call or
  * batched with others.  There is no seed: reproducing OpenCV's sample sequence is the point.

@@ -98,6 +98,33 @@ def _vp(x):
     return C.c_void_p(x)
 
 
+def flatten_matches(q_list, t_list):
+    """Per-pair match lists (queryIdx / trainIdx arrays, one of each per pair) -> (match_q int32, match_t int32, match_off int64
+    [len(q_list) + 1]), the concatenated form the *_pairs calls take."""
+    if len(q_list) != len(t_list) or any(len(q) != len(t) for q, t in zip(q_list, t_list)):
+        raise ValueError("flatten_matches: every pair needs as many query as train indices")
+    off = np.zeros(len(q_list) + 1, np.int64); off[1:] = np.cumsum([len(q) for q in q_list])
+    cat = lambda xs: np.concatenate([np.asarray(x, np.int32) for x in xs]) if len(xs) else np.zeros(0, np.int32)
+    return cat(q_list), cat(t_list), off
+
+
+def _pair_batch_args(points, pairs, match_q, match_t, match_off):
+    """The image-pair batch arrays of include/sfmb200.h as ctypes arguments, in the C order pts, img_off, n_img, pairs, n_pairs,
+    match_q, match_t, match_off; and the numbers of pairs and matches.  The arrays are kept alive by the returned pointers."""
+    pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
+    img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
+    allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
+    pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+    mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
+    moff = np.ascontiguousarray(match_off, np.int64)
+    P = pairs.shape[0]
+    if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
+        raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+    args = (_p(allp, C.c_float), _p(img_off, C.c_int32), len(pts), _p(pairs, C.c_int32), P, _p(mq, C.c_int32), _p(mt, C.c_int32),
+            _p(moff, C.c_int64))
+    return args, P, mq.shape[0]
+
+
 class Context:
     """sfmb200_ctx: one per GPU."""
 
@@ -188,23 +215,13 @@ class Context:
         owning match_off[p]:match_off[p+1]).  poses [P, 2, 3, 4]: pair p's (Pleft, Pright).
         Returns (X [sum of matches, 3], keep [sum of matches], n_keep [P])."""
         K = np.ascontiguousarray(K, np.float32).reshape(9)
-        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
-        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
-        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
-        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
-        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
-        moff = np.ascontiguousarray(match_off, np.int64)
-        P = pairs.shape[0]
+        batch, P, M = _pair_batch_args(points, pairs, match_q, match_t, match_off)
         poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 24)
-        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
-            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
         if poses.shape[0] != P:
             raise ValueError("poses must hold one (Pleft, Pright) per pair")
-        M = mq.shape[0]
         X = np.empty((max(M, 1), 3), np.float32); keep = np.empty(max(M, 1), np.uint8); nk = np.zeros(max(P, 1), np.int32)
-        self._check(lib().sfmb200_triangulate_pairs(self._h, _p(K, C.c_float), _p(poses, C.c_float), _p(allp, C.c_float), _p(img_off, C.c_int32),
-                                                    len(pts), _p(pairs, C.c_int32), P, _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64),
-                                                    C.c_float(max_reproj), _p(X, C.c_float), _p(keep, C.c_uint8), _p(nk, C.c_int32)))
+        self._check(lib().sfmb200_triangulate_pairs(self._h, _p(K, C.c_float), _p(poses, C.c_float), *batch, C.c_float(max_reproj),
+                                                    _p(X, C.c_float), _p(keep, C.c_uint8), _p(nk, C.c_int32)))
         return X[:M], keep[:M], nk[:P]
 
     def triangulate_device(self, K, Pl, Pr, d_left, d_right, d_mq, d_mt, m, d_X, d_keep, d_nkeep, max_reproj=MIN_REPROJECTION_ERROR):
@@ -278,24 +295,14 @@ class Context:
         Returns (E [P, 3, 3], R [P, 3, 3], t [P, 3], inlier_mask [sum of matches], pose_mask [sum of matches], summary dict of
         arrays found / n_inliers / n_good / iterations / n_samples / n_hypotheses [P])."""
         K = np.ascontiguousarray(K, np.float32).reshape(9)
-        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
-        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
-        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
-        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
-        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
-        moff = np.ascontiguousarray(match_off, np.int64)
-        P = pairs.shape[0]
-        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
-            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+        batch, P, M = _pair_batch_args(points, pairs, match_q, match_t, match_off)
         o = options or essential_default_options(**kw)
         E = np.zeros((max(P, 1), 9)); Rm = np.zeros((max(P, 1), 9)); t = np.zeros((max(P, 1), 3))
-        inl = np.zeros(max(mq.shape[0], 1), np.uint8); pm = np.zeros(max(mq.shape[0], 1), np.uint8); s = (EssentialSummary * max(P, 1))()
-        self._check(lib().sfmb200_find_camera_matrices_pairs(self._h, _p(K, C.c_float), _p(allp, C.c_float), _p(img_off, C.c_int32), len(pts),
-                                                             _p(pairs, C.c_int32), P, _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64),
-                                                             C.byref(o), _p(E, C.c_double), _p(Rm, C.c_double), _p(t, C.c_double),
-                                                             _p(inl, C.c_uint8), _p(pm, C.c_uint8), s))
+        inl = np.zeros(max(M, 1), np.uint8); pm = np.zeros(max(M, 1), np.uint8); s = (EssentialSummary * max(P, 1))()
+        self._check(lib().sfmb200_find_camera_matrices_pairs(self._h, _p(K, C.c_float), *batch, C.byref(o), _p(E, C.c_double), _p(Rm, C.c_double),
+                                                             _p(t, C.c_double), _p(inl, C.c_uint8), _p(pm, C.c_uint8), s))
         summ = {k: np.array([getattr(s[p], k) for p in range(P)], np.int32) for k, _ in EssentialSummary._fields_}
-        return E[:P].reshape(P, 3, 3), Rm[:P].reshape(P, 3, 3), t[:P], inl[:mq.shape[0]], pm[:mq.shape[0]], summ
+        return E[:P].reshape(P, 3, 3), Rm[:P].reshape(P, 3, 3), t[:P], inl[:M], pm[:M], summ
 
     def five_point(self, x1, x2):
         """sfmb200_five_point: x1, x2 [ns, 5, 2] normalised coordinates -> (E [ns, 10, 3, 3], nsol [ns])."""
@@ -323,22 +330,12 @@ class Context:
         options: HomographyOptions or keyword overrides of the defaults (max_iters, confidence, threshold_px, refine_iters,
         record_trace).  Returns (H [P, 3, 3], mask [sum of matches] uint8, summary dict of arrays found / n_inliers /
         ransac_inliers / iterations [P])."""
-        pts = [np.ascontiguousarray(p, np.float32).reshape(-1, 2) for p in points]
-        img_off = np.zeros(len(pts) + 1, np.int32); img_off[1:] = np.cumsum([len(p) for p in pts])
-        allp = np.ascontiguousarray(np.concatenate(pts, 0)) if pts else np.zeros((0, 2), np.float32)
-        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
-        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
-        moff = np.ascontiguousarray(match_off, np.int64)
-        P = pairs.shape[0]
-        if moff.shape[0] != P + 1 or mq.shape != mt.shape or (P and moff[-1] != mq.shape[0]):
-            raise ValueError("match_off must have len(pairs) + 1 entries ending at the number of matches")
+        batch, P, M = _pair_batch_args(points, pairs, match_q, match_t, match_off)
         o = options or homography_default_options(**kw)
-        H = np.zeros((max(P, 1), 9)); mask = np.zeros(max(mq.shape[0], 1), np.uint8); s = (HomographySummary * max(P, 1))()
-        self._check(lib().sfmb200_find_homography_pairs(self._h, _p(allp, C.c_float), _p(img_off, C.c_int32), len(pts), _p(pairs, C.c_int32), P,
-                                                        _p(mq, C.c_int32), _p(mt, C.c_int32), _p(moff, C.c_int64), C.byref(o), _p(H, C.c_double),
-                                                        _p(mask, C.c_uint8), s))
+        H = np.zeros((max(P, 1), 9)); mask = np.zeros(max(M, 1), np.uint8); s = (HomographySummary * max(P, 1))()
+        self._check(lib().sfmb200_find_homography_pairs(self._h, *batch, C.byref(o), _p(H, C.c_double), _p(mask, C.c_uint8), s))
         summ = {k: np.array([getattr(s[p], k) for p in range(P)], np.int32) for k, _ in HomographySummary._fields_}
-        return H[:P].reshape(P, 3, 3), mask[:mq.shape[0]], summ
+        return H[:P].reshape(P, 3, 3), mask[:M], summ
 
     def homography_last_trace(self, pair):
         """sfmb200_homography_last_trace: (quads [V, 4], RANSAC counts [V]) visited for `pair` by the last find_homography_pairs call

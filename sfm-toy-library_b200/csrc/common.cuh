@@ -134,6 +134,16 @@ struct sfmb200_ctx {
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);
 
+// Host-side input checks shared by several entry points (ctx.cu).  Each returns SFMB200_OK, or SFMB200_ERR_INVALID with the
+// message set through sfmb200_fail.
+// check_pair_batch: the image-pair batch layout of include/sfmb200.h (pts / img_off / pairs / match_q / match_t / match_off) with
+// at most max_matches matches; on success *n_matches = match_off[n_pairs], or 0 when n_pairs == 0.
+int check_pair_batch(sfmb200_ctx* ctx, const float* pts, const int32_t* img_off, int n_img, const int32_t* pairs, int n_pairs,
+                     const int32_t* match_q, const int32_t* match_t, const int64_t* match_off, int64_t max_matches, int64_t* n_matches);
+// check_two_view_matches: match_q / match_t [m] of a single-pair call index pts_left [n_left] / pts_right [n_right]; both NULL
+// means identity alignment, which needs m <= min(n_left, n_right).
+int check_two_view_matches(sfmb200_ctx* ctx, const int32_t* match_q, const int32_t* match_t, int m, int n_left, int n_right);
+
 #define SFM_CUDA(ctx, call)                                                                              \
     do {                                                                                                 \
         cudaError_t e_ = (call);                                                                         \

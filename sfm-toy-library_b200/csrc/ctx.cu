@@ -10,6 +10,42 @@ int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...) {
     return code;
 }
 
+int check_pair_batch(sfmb200_ctx* ctx, const float* pts, const int32_t* img_off, int n_img, const int32_t* pairs, int n_pairs,
+                     const int32_t* match_q, const int32_t* match_t, const int64_t* match_off, int64_t max_matches, int64_t* n_matches) {
+    if (!img_off || (n_pairs > 0 && (!pairs || !match_off))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    if (img_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off[0] must be 0");
+    for (int i = 0; i < n_img; ++i)
+        if (img_off[i + 1] < img_off[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off is not monotone at image %d", i);
+    if (img_off[n_img] > 0 && !pts) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    if (n_pairs > 0 && match_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off[0] must be 0");
+    for (int p = 0; p < n_pairs; ++p) {
+        if (match_off[p + 1] < match_off[p]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off is not monotone at pair %d", p);
+        if (pairs[2 * p] < 0 || pairs[2 * p] >= n_img || pairs[2 * p + 1] < 0 || pairs[2 * p + 1] >= n_img)
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "pair %d names an image outside [0, %d)", p, n_img);
+    }
+    const int64_t M = n_pairs > 0 ? match_off[n_pairs] : 0;
+    if (M > max_matches) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "too many matches in one call");
+    if (M > 0 && (!match_q || !match_t)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    for (int p = 0; p < n_pairs; ++p) {
+        const int nl = img_off[pairs[2 * p] + 1] - img_off[pairs[2 * p]], nr = img_off[pairs[2 * p + 1] + 1] - img_off[pairs[2 * p + 1]];
+        for (int64_t k = match_off[p]; k < match_off[p + 1]; ++k)
+            if (match_q[k] < 0 || match_q[k] >= nl || match_t[k] < 0 || match_t[k] >= nr)
+                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %lld of pair %d indexes outside its images' key points", (long long)k, p);
+    }
+    *n_matches = M;
+    return SFMB200_OK;
+}
+
+int check_two_view_matches(sfmb200_ctx* ctx, const int32_t* match_q, const int32_t* match_t, int m, int n_left, int n_right) {
+    if ((match_q == nullptr) != (match_t == nullptr)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_q and match_t must both be given or both be NULL");
+    if (!match_q && (m > n_left || m > n_right)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "identity alignment needs m <= min(n_left, n_right)");
+    if (match_q)
+        for (int i = 0; i < m; ++i)
+            if (match_q[i] < 0 || match_q[i] >= n_left || match_t[i] < 0 || match_t[i] >= n_right)
+                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %d indexes outside the keypoint arrays", i);
+    return SFMB200_OK;
+}
+
 extern "C" {
 
 int sfmb200_version(void) { return SFMB200_VERSION; }

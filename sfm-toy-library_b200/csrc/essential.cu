@@ -397,12 +397,7 @@ int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* 
     if (inlier_mask) memset(inlier_mask, 0, (size_t)m);
     if (pose_mask) memset(pose_mask, 0, (size_t)m);
     if (m > 0 && (!pts_left || !pts_right)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if ((match_q == nullptr) != (match_t == nullptr)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_q and match_t must both be given or both be NULL");
-    if (!match_q && (m > n_left || m > n_right)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "identity alignment needs m <= min(n_left, n_right)");
-    if (match_q)
-        for (int i = 0; i < m; ++i)
-            if (match_q[i] < 0 || match_q[i] >= n_left || match_t[i] < 0 || match_t[i] >= n_right)
-                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %d indexes outside the keypoint arrays", i);
+    if (const int rc = check_two_view_matches(ctx, match_q, match_t, m, n_left, n_right)) return rc;
     if (m < 5) return SFMB200_OK;
     const int64_t moff[2] = {0, m};
     return es_run(ctx, o, focal, cx, cy, 1, moff, [&](float* ha, float* hb) {
@@ -426,26 +421,8 @@ int sfmb200_find_camera_matrices_pairs(sfmb200_ctx* ctx, const float* K, const f
     const double focal = (double)K[0], cx = (double)K[2], cy = (double)K[5];
     if (!(focal != 0.0) || !std::isfinite(focal) || !std::isfinite(cx) || !std::isfinite(cy)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "K: focal length must be finite and nonzero");
     if (n_pairs == 0) return SFMB200_OK;
-    if (!img_off || !pairs || !match_off) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (img_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off[0] must be 0");
-    for (int i = 0; i < n_img; ++i)
-        if (img_off[i + 1] < img_off[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off is not monotone at image %d", i);
-    if (img_off[n_img] > 0 && !pts) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (match_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off[0] must be 0");
-    for (int p = 0; p < n_pairs; ++p) {
-        if (match_off[p + 1] < match_off[p]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off is not monotone at pair %d", p);
-        if (pairs[2 * p] < 0 || pairs[2 * p] >= n_img || pairs[2 * p + 1] < 0 || pairs[2 * p + 1] >= n_img)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "pair %d names an image outside [0, %d)", p, n_img);
-    }
-    const int64_t M = match_off[n_pairs];
-    if (M > INT32_MAX / 2) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "too many matches in one call");
-    if (M > 0 && (!match_q || !match_t)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    for (int p = 0; p < n_pairs; ++p) {
-        const int nl = img_off[pairs[2 * p] + 1] - img_off[pairs[2 * p]], nr = img_off[pairs[2 * p + 1] + 1] - img_off[pairs[2 * p + 1]];
-        for (int64_t k = match_off[p]; k < match_off[p + 1]; ++k)
-            if (match_q[k] < 0 || match_q[k] >= nl || match_t[k] < 0 || match_t[k] >= nr)
-                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %lld of pair %d indexes outside its images' key points", (long long)k, p);
-    }
+    int64_t M = 0;
+    if (const int rc = check_pair_batch(ctx, pts, img_off, n_img, pairs, n_pairs, match_q, match_t, match_off, INT32_MAX / 2, &M)) return rc;
     if (summary) memset(summary, 0, sizeof(sfmb200_essential_summary) * (size_t)n_pairs);
     if (E) memset(E, 0, 9 * sizeof(double) * (size_t)n_pairs);
     if (R) memset(R, 0, 9 * sizeof(double) * (size_t)n_pairs);

@@ -289,27 +289,9 @@ int sfmb200_find_homography_pairs(sfmb200_ctx* ctx, const float* pts, const int3
     if (o.max_iters < 1 || !(o.confidence > 0.0 && o.confidence < 1.0) || !(o.threshold_px > 0.0) || o.refine_iters < 1 ||
         (o.record_trace != 0 && o.record_trace != 1))
         return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "homography options: max_iters >= 1, confidence in (0, 1), threshold_px > 0, refine_iters >= 1, record_trace 0 or 1");
-    if (!img_off || (n_pairs > 0 && (!pairs || !match_off))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (img_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off[0] must be 0");
-    for (int i = 0; i < n_img; ++i)
-        if (img_off[i + 1] < img_off[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off is not monotone at image %d", i);
+    int64_t M = 0;
+    if (const int rc = check_pair_batch(ctx, pts, img_off, n_img, pairs, n_pairs, match_q, match_t, match_off, INT32_MAX / 2, &M)) return rc;
     const int64_t n_pts = img_off[n_img];
-    if (n_pts > 0 && !pts) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (n_pairs > 0 && match_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off[0] must be 0");
-    for (int p = 0; p < n_pairs; ++p) {
-        if (match_off[p + 1] < match_off[p]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off is not monotone at pair %d", p);
-        if (pairs[2 * p] < 0 || pairs[2 * p] >= n_img || pairs[2 * p + 1] < 0 || pairs[2 * p + 1] >= n_img)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "pair %d names an image outside [0, %d)", p, n_img);
-    }
-    const int64_t M = n_pairs > 0 ? match_off[n_pairs] : 0;
-    if (M > INT32_MAX / 2) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "too many matches in one call");
-    if (M > 0 && (!match_q || !match_t)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    for (int p = 0; p < n_pairs; ++p) {
-        const int nl = img_off[pairs[2 * p] + 1] - img_off[pairs[2 * p]], nr = img_off[pairs[2 * p + 1] + 1] - img_off[pairs[2 * p + 1]];
-        for (int64_t k = match_off[p]; k < match_off[p + 1]; ++k)
-            if (match_q[k] < 0 || match_q[k] >= nl || match_t[k] < 0 || match_t[k] >= nr)
-                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %lld of pair %d indexes outside its images' key points", (long long)k, p);
-    }
     if ((size_t)n_pairs * (size_t)o.max_iters > (size_t)INT32_MAX / 4 && o.record_trace)
         return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "trace too large: n_pairs * max_iters");
     if (summary) memset(summary, 0, sizeof(sfmb200_homography_summary) * (size_t)n_pairs);

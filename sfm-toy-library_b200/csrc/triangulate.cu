@@ -153,12 +153,7 @@ int sfmb200_triangulate(sfmb200_ctx* ctx, const float* K, const float* Pl, const
     if (n_keep) *n_keep = 0;
     if (m == 0) return SFMB200_OK;
     if (!pts_left || !pts_right || !X || !keep) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if ((match_q == nullptr) != (match_t == nullptr)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_q and match_t must both be given or both be NULL");
-    if (!match_q && (m > n_left || m > n_right)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "identity alignment needs m <= min(n_left, n_right)");
-    if (match_q)
-        for (int i = 0; i < m; ++i)
-            if (match_q[i] < 0 || match_q[i] >= n_left || match_t[i] < 0 || match_t[i] >= n_right)
-                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %d indexes outside the keypoint arrays", i);
+    if (const int rc = check_two_view_matches(ctx, match_q, match_t, m, n_left, n_right)) return rc;
     std::lock_guard<std::mutex> lk(ctx->mu);
     SFM_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t bytes = Carver::pad(8 * (size_t)n_left) + Carver::pad(8 * (size_t)n_right) + 2 * Carver::pad(4 * (size_t)m) +
@@ -191,26 +186,10 @@ int sfmb200_triangulate_pairs(sfmb200_ctx* ctx, const float* K, const float* pos
                               float max_reproj_px, float* X, uint8_t* keep, int32_t* n_keep) {
     if (!ctx || n_img < 0 || n_pairs < 0) return SFMB200_ERR_INVALID;
     if (n_pairs == 0) return SFMB200_OK;
-    if (!K || !poses || !img_off || !pairs || !match_off) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (img_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off[0] must be 0");
-    for (int i = 0; i < n_img; ++i)
-        if (img_off[i + 1] < img_off[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "img_off is not monotone at image %d", i);
-    if (img_off[n_img] > 0 && !pts) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    if (match_off[0] != 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off[0] must be 0");
-    for (int p = 0; p < n_pairs; ++p) {
-        if (match_off[p + 1] < match_off[p]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match_off is not monotone at pair %d", p);
-        if (pairs[2 * p] < 0 || pairs[2 * p] >= n_img || pairs[2 * p + 1] < 0 || pairs[2 * p + 1] >= n_img)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "pair %d names an image outside [0, %d)", p, n_img);
-    }
-    const int64_t M = match_off[n_pairs];
-    if (M > INT32_MAX) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "too many matches in one call");
-    if (M > 0 && (!match_q || !match_t || !X || !keep)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
-    for (int p = 0; p < n_pairs; ++p) {
-        const int nl = img_off[pairs[2 * p] + 1] - img_off[pairs[2 * p]], nr = img_off[pairs[2 * p + 1] + 1] - img_off[pairs[2 * p + 1]];
-        for (int64_t k = match_off[p]; k < match_off[p + 1]; ++k)
-            if (match_q[k] < 0 || match_q[k] >= nl || match_t[k] < 0 || match_t[k] >= nr)
-                return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "match %lld of pair %d indexes outside its images' key points", (long long)k, p);
-    }
+    if (!K || !poses) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    int64_t M = 0;
+    if (const int rc = check_pair_batch(ctx, pts, img_off, n_img, pairs, n_pairs, match_q, match_t, match_off, INT32_MAX, &M)) return rc;
+    if (M > 0 && (!X || !keep)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
     if (n_keep) memset(n_keep, 0, sizeof(int32_t) * (size_t)n_pairs);
     if (M == 0) return SFMB200_OK;
     const int64_t NP = img_off[n_img];

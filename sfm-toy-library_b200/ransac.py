@@ -80,8 +80,7 @@ def homographyInliersAllPairs(features, pairs, matches, ctx=None):
     ctx = ctx or default_context()
     if len(pairs) == 0:
         return np.zeros(0, np.int64)
-    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
-    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
+    mq, mt, off = capi.flatten_matches([m["queryIdx"] for m in matches], [m["trainIdx"] for m in matches])
     _, _, s = ctx.find_homography_pairs([f.points for f in features], pairs, mq, mt, off, threshold_px=RANSAC_THRESHOLD)
     return np.where(s["found"] != 0, s["n_inliers"], 0).astype(np.int64)
 
@@ -134,9 +133,8 @@ def cameraMatricesManyPairs(intrinsics: Intrinsics, features, pairs, matches, ct
     ctx = ctx or default_context()
     if len(pairs) == 0:
         return []
-    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
-    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
-    _, R, t, _, pose_mask, s = ctx.find_camera_matrices_pairs(intrinsics.K, [f.points for f in features], pairs, mq, mt, off, seed=seed)
+    mq, mt, off = capi.flatten_matches([m["queryIdx"] for m in matches], [m["trainIdx"] for m in matches])
+    _, R, t, _, pose_mask, s =ctx.find_camera_matrices_pairs(intrinsics.K, [f.points for f in features], pairs, mq, mt, off, seed=seed)
     out = []
     for p, m in enumerate(matches):
         Pleft = np.eye(3, 4, dtype=np.float32)

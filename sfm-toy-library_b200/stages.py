@@ -144,9 +144,8 @@ def triangulateManyPairs(intrinsics: Intrinsics, features: List[Features], pairs
     ctx = ctx or default_context()
     if len(pairs) == 0:
         return []
-    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in matches])
-    mq = np.concatenate([np.asarray(m["queryIdx"], np.int32) for m in matches]); mt = np.concatenate([np.asarray(m["trainIdx"], np.int32) for m in matches])
-    X, keep, _ = ctx.triangulate_pairs(intrinsics.K, [np.stack([Pl, Pr]) for Pl, Pr in poses], [f.points for f in features], pairs, mq, mt, off,
+    mq, mt, off = capi.flatten_matches([m["queryIdx"] for m in matches], [m["trainIdx"] for m in matches])
+    X, keep, _ =ctx.triangulate_pairs(intrinsics.K, [np.stack([Pl, Pr]) for Pl, Pr in poses], [f.points for f in features], pairs, mq, mt, off,
                                        capi.MIN_REPROJECTION_ERROR)
     clouds = []
     for p, (left, right) in enumerate(pairs):

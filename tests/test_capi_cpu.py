@@ -70,6 +70,21 @@ def test_flatten_bundle_follows_reference_assembly_order(L):
     assert cams.shape == (3, 6) and np.all(cams == 0)
 
 
+def test_flatten_matches():
+    """per-pair match lists -> the match_q / match_t / match_off arrays of the *_pairs calls"""
+    mq, mt, off = capi.flatten_matches([], [])
+    assert (mq.dtype, mt.dtype, off.dtype) == (np.int32, np.int32, np.int64)
+    assert mq.shape == mt.shape == (0,) and off.tolist() == [0]
+    from sfm_toy_library_b200 import stages
+    m = np.zeros(2, stages.DMATCH); m["queryIdx"] = [4, 0]; m["trainIdx"] = [1, 3]
+    mq, mt, off = capi.flatten_matches([m["queryIdx"], np.zeros(0, np.int64), [7], m["queryIdx"][:0]],
+                                       [m["trainIdx"], np.zeros(0), np.array([5], np.uint16), m["trainIdx"][:0]])
+    assert (mq.dtype, mt.dtype, off.dtype) == (np.int32, np.int32, np.int64)
+    assert mq.tolist() == [4, 0, 7] and mt.tolist() == [1, 3, 5] and off.tolist() == [0, 2, 2, 3, 3]
+    with pytest.raises(ValueError):
+        capi.flatten_matches([[1, 2]], [[1]])
+
+
 def _naive_validate(nc, obs_cam, pt_off):
     """The obvious nested loop (what the library's slow path and the previous implementation do)."""
     np_, nobs = len(pt_off) - 1, len(obs_cam)

@@ -1,8 +1,7 @@
 """Essential-matrix RANSAC and pose recovery for many image pairs in one call (sfmb200_find_camera_matrices_pairs): every pair's
 outputs bitwise equal to the single-pair call, whatever else is in the batch; the per-pair edge cases; a batch larger than one group
-of the hypothesis budget; the host-side refusals; and the runSfM replay with the batched stage injected."""
-import ctypes as C
-
+of the hypothesis budget; the refusals of options and K; and the runSfM replay with the batched stage injected.  The host-side
+refusals of the batch layout are in test_gpu_pair_batch.py."""
 import numpy as np
 import pytest
 
@@ -26,16 +25,10 @@ def cfg1():
     return Cfg1()
 
 
-def _flatten(q_list, t_list):
-    off = np.zeros(len(q_list) + 1, np.int64); off[1:] = np.cumsum([len(q) for q in q_list])
-    cat = lambda xs: np.concatenate([np.asarray(x, np.int32) for x in xs]) if xs else np.zeros(0, np.int32)
-    return cat(q_list), cat(t_list), off
-
-
 def _crazyhorse(cfg1, order):
     pts = [f.points for f in cfg1.features]
     pairs = [cfg1.pairs[p] for p in order]
-    mq, mt, off = _flatten([cfg1.matches[p][0] for p in order], [cfg1.matches[p][1] for p in order])
+    mq, mt, off = capi.flatten_matches([cfg1.matches[p][0] for p in order], [cfg1.matches[p][1] for p in order])
     return pts, pairs, mq, mt, off
 
 
@@ -69,7 +62,7 @@ def test_mixed_batch(ctx):
     cases = [((0, 1), ident(0)), ((0, 1), ident(300)), ((0, 1), ident(1)), ((2, 3), ident(30)), ((0, 1), ident(4)),
              ((0, 1), ident(5)), ((1, 0), ident(200)), ((0, 1), ident(0))]
     pairs = [c[0] for c in cases]
-    mq, mt, off = _flatten([c[1][0] for c in cases], [c[1][1] for c in cases])
+    mq, mt, off = capi.flatten_matches([c[1][0] for c in cases], [c[1][1] for c in cases])
     out = ctx.find_camera_matrices_pairs(K, pts, pairs, mq, mt, off)
     s = out[5]
     np.testing.assert_array_equal(s["found"], [0, 1, 0, 0, 0, 1, 1, 0])
@@ -90,7 +83,7 @@ def test_batch_larger_than_one_hypothesis_group(ctx):
     for k in range(300):
         a, b, Rt, tt, _ = synthetic_scene(1000 + k, int(rs.randint(800, 1201)), noise_px=0.5, outliers=0.3)
         pts += [a, b]; pairs.append((2 * k, 2 * k + 1)); qs.append(np.arange(len(a))); truth.append((Rt, tt))
-    mq, mt, off = _flatten(qs, qs)
+    mq, mt, off = capi.flatten_matches(qs, qs)
     l0 = ctx.kernel_launches
     out = ctx.find_camera_matrices_pairs(K, pts, pairs, mq, mt, off, seed=3)
     assert ctx.kernel_launches - l0 == 2 * 3 + 2             # solve, score, select per group; cheirality and pose once
@@ -103,42 +96,20 @@ def test_batch_larger_than_one_hypothesis_group(ctx):
     _assert_equal_to_single_calls(ctx, pts, pairs, mq, mt, off, out, which, seed=3)
 
 
-def _raw(ctx, pts, img_off, pairs, mq, mt, moff, K_=K, **kw):
-    """the C call with the caller's own offsets (the binding derives img_off itself)"""
-    allp = np.ascontiguousarray(np.concatenate(pts), np.float32); img_off = np.asarray(img_off, np.int32)
-    pairs = np.asarray(pairs, np.int32).reshape(-1, 2); mq = np.asarray(mq, np.int32); mt = np.asarray(mt, np.int32)
-    moff = np.asarray(moff, np.int64); Kf = np.ascontiguousarray(K_, np.float32).reshape(9)
-    P = len(pairs); M = max(len(mq), 1)
-    E = np.zeros((max(P, 1), 9)); inl = np.zeros(M, np.uint8); s = (capi.EssentialSummary * max(P, 1))()
-    o = capi.essential_default_options(**kw)
-    ptr = lambda x, tp: x.ctypes.data_as(C.POINTER(tp))
-    ctx._check(capi.lib().sfmb200_find_camera_matrices_pairs(ctx._h, ptr(Kf, C.c_float), ptr(allp, C.c_float), ptr(img_off, C.c_int32), len(img_off) - 1,
-                                                             ptr(pairs, C.c_int32), P, ptr(mq, C.c_int32), ptr(mt, C.c_int32), ptr(moff, C.c_int64),
-                                                             C.byref(o), ptr(E, C.c_double), None, None, ptr(inl, C.c_uint8), None, s))
-    return s[0].found
-
-
 def test_invalid_inputs_are_refused_and_the_context_stays_usable(ctx):
+    """the options and K of the single call; the refusals of the batch layout are in test_gpu_pair_batch.py"""
     a, b, *_ = synthetic_scene(5, 60)
-    pts = [a, b]; idx = np.arange(60)
-    good = dict(img_off=[0, 60, 120], pairs=[(0, 1)], mq=idx, mt=idx, moff=[0, 60])
-    assert _raw(ctx, pts, **good) == 1
-    bad = [(dict(pairs=[(0, 2)]), "outside \\[0, 2\\)"),
-           (dict(pairs=[(-1, 1)]), "outside \\[0, 2\\)"),
-           (dict(img_off=[0, 70, 60]), "img_off is not monotone"),
-           (dict(img_off=[1, 60, 120]), "img_off\\[0\\] must be 0"),
-           (dict(pairs=[(0, 1), (0, 1)], moff=[0, 60, 30]), "match_off is not monotone"),
-           (dict(moff=[5, 60]), "match_off\\[0\\] must be 0"),
-           (dict(mq=np.r_[idx[:59], 60]), "indexes outside its images"),
-           (dict(mt=np.r_[-1, idx[1:]]), "indexes outside its images"),
-           (dict(confidence=1.0), "essential options"),
-           (dict(max_iters=0), "essential options"),
-           (dict(K_=np.zeros((3, 3))), "focal length")]
-    for change, msg in bad:
+    idx = np.arange(60)
+    good = ([a, b], [(0, 1)], idx, idx, [0, 60])
+    assert ctx.find_camera_matrices_pairs(K, *good)[5]["found"][0] == 1
+    bad = [(K, dict(confidence=1.0), "essential options"),
+           (K, dict(max_iters=0), "essential options"),
+           (np.zeros((3, 3)), {}, "focal length")]
+    for K_, kw, msg in bad:
         with pytest.raises(capi.SfmB200Error, match=msg):
-            _raw(ctx, pts, **{**good, **change})
-        assert _raw(ctx, pts, **good) == 1
-    E, R, t, inl, pm, s = ctx.find_camera_matrices_pairs(K, pts, np.zeros((0, 2)), np.zeros(0), np.zeros(0), [0])
+            ctx.find_camera_matrices_pairs(K_, *good, **kw)
+        assert ctx.find_camera_matrices_pairs(K, *good)[5]["found"][0] == 1
+    E, R, t, inl, pm, s = ctx.find_camera_matrices_pairs(K, [a, b], np.zeros((0, 2)), np.zeros(0), np.zeros(0), [0])
     assert E.shape == (0, 3, 3) and len(s["found"]) == 0
 
 

@@ -24,11 +24,10 @@ def ctx():
 
 def _batch(ctx, pairs_ab, **kw):
     """Each (a, b) as its own two images, all pairs in one call."""
-    pts = []; pairs = []; mq = []; mt = []; off = [0]
-    for k, (a, b) in enumerate(pairs_ab):
-        pts += [a, b]; pairs.append((2 * k, 2 * k + 1))
-        mq.append(np.arange(len(a), dtype=np.int32)); mt.append(np.arange(len(b), dtype=np.int32)); off.append(off[-1] + len(a))
-    return ctx.find_homography_pairs(pts, pairs, np.concatenate(mq), np.concatenate(mt), np.array(off), **kw), off
+    pts = [x for a, b in pairs_ab for x in (a, b)]
+    pairs = [(2 * k, 2 * k + 1) for k in range(len(pairs_ab))]
+    mq, mt, off = capi.flatten_matches([np.arange(len(a)) for a, _ in pairs_ab], [np.arange(len(b)) for _, b in pairs_ab])
+    return ctx.find_homography_pairs(pts, pairs, mq, mt, off, **kw), off
 
 
 def _check_against_cv2(ctx, names, pairs_ab, off, H, mask, s):
@@ -80,8 +79,7 @@ def test_single_and_batched_calls_are_identical(ctx):
 def test_indexed_points_and_validation(ctx):
     cfg = Cfg1()
     pairs = cfg.pairs
-    off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m[0]) for m in cfg.matches])
-    mq = np.concatenate([m[0] for m in cfg.matches]); mt = np.concatenate([m[1] for m in cfg.matches])
+    mq, mt, off = capi.flatten_matches([m[0] for m in cfg.matches], [m[1] for m in cfg.matches])
     H, mask, s = ctx.find_homography_pairs([f.points for f in cfg.features], pairs, mq, mt, off)
     for p, (a, b) in enumerate(crazyhorse_pairs(cfg)):
         _, mc = cv2.findHomography(a, b, cv2.RANSAC, 10.0)

@@ -1,8 +1,7 @@
 """Two-view triangulation for many image pairs in one call (sfmb200_triangulate_pairs): every pair's X, keep and n_keep bitwise
 equal to the single-pair call, whatever else is in the batch; the crazyhorse calls against their goldens; a 1225-pair synthetic
-batch against the oracle; the edge cases; the host-side refusals; and the runSfM replay with the batched stage injected."""
-import ctypes as C
-
+batch against the oracle; the edge cases; the binding's refusals; and the runSfM replay with the batched stage injected.  The
+host-side refusals of the C call are in test_gpu_pair_batch.py."""
 import numpy as np
 import pytest
 
@@ -24,12 +23,6 @@ def ctx():
 @pytest.fixture(scope="module")
 def cfg1():
     return Cfg1()
-
-
-def _flatten(q_list, t_list):
-    off = np.zeros(len(q_list) + 1, np.int64); off[1:] = np.cumsum([len(q) for q in q_list])
-    cat = lambda xs: np.concatenate([np.asarray(x, np.int32) for x in xs]) if xs else np.zeros(0, np.int32)
-    return cat(q_list), cat(t_list), off
 
 
 def _assert_equal_to_single_calls(ctx, K, poses, pts, pairs, mq, mt, off, out, which=None):
@@ -56,7 +49,7 @@ def _cfg1_batch(cfg1, calls, K=None):
     cs = [cfg1.tri(k) for k in calls]
     pairs = [tuple(int(x) for x in c["pair"]) for c in cs]
     poses = [(c["Pl"], c["Pr"]) for c in cs]
-    mq, mt, off = _flatten([c["mq"] for c in cs], [c["mt"] for c in cs])
+    mq, mt, off = capi.flatten_matches([c["mq"] for c in cs], [c["mt"] for c in cs])
     return (cs[0]["K"] if K is None else K), poses, [f.points for f in cfg1.features], pairs, mq, mt, off
 
 
@@ -116,22 +109,6 @@ def test_synthetic_1225_pairs(ctx, oracle):
         assert (np.abs(np.max(eo[diff], axis=1) - 10.0) < ERR_TOL).all()
 
 
-def _raw(ctx, K, poses, pts, img_off, pairs, mq, mt, moff, with_nkeep=True):
-    """the C call with the caller's own offsets (the binding derives img_off itself); returns (X, keep, n_keep or None)"""
-    allp = np.ascontiguousarray(np.concatenate(pts), np.float32); img_off = np.asarray(img_off, np.int32)
-    pairs = np.asarray(pairs, np.int32).reshape(-1, 2); mq = np.asarray(mq, np.int32); mt = np.asarray(mt, np.int32)
-    moff = np.asarray(moff, np.int64); Kf = np.ascontiguousarray(K, np.float32).reshape(9)
-    poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 24)
-    P = len(pairs); M = max(len(mq), 1)
-    X = np.full((M, 3), np.nan, np.float32); keep = np.full(M, 7, np.uint8); nk = np.full(max(P, 1), -1, np.int32)
-    ptr = lambda x, tp: x.ctypes.data_as(C.POINTER(tp))
-    ctx._check(capi.lib().sfmb200_triangulate_pairs(ctx._h, ptr(Kf, C.c_float), ptr(poses, C.c_float), ptr(allp, C.c_float), ptr(img_off, C.c_int32),
-                                                    len(img_off) - 1, ptr(pairs, C.c_int32), P, ptr(mq, C.c_int32), ptr(mt, C.c_int32),
-                                                    ptr(moff, C.c_int64), C.c_float(10.0), ptr(X, C.c_float), ptr(keep, C.c_uint8),
-                                                    ptr(nk, C.c_int32) if with_nkeep else None))
-    return X[:len(mq)], keep[:len(mq)], (nk[:P] if with_nkeep else None)
-
-
 def _two_views(cfg1):
     c = cfg1.tri(4)
     i, j = (int(x) for x in c["pair"])
@@ -149,47 +126,34 @@ def test_edge_cases(ctx, cfg1):
              ((2, 1), (ends_a[::-1], ends_b[::-1])), ((1, 2), (np.r_[nb - 1, 0], np.r_[na - 1, 0])), ((0, 1), (np.zeros(0), np.zeros(0)))]
     pairs = [c[0] for c in cases]
     poses = [(Pl, Pr)] * len(cases)
-    mq, mt, off = _flatten([c[1][0] for c in cases], [c[1][1] for c in cases])
+    mq, mt, off = capi.flatten_matches([c[1][0] for c in cases], [c[1][1] for c in cases])
     out = ctx.triangulate_pairs(K, poses, pts, pairs, mq, mt, off)
     assert out[2][0] == out[2][2] == out[2][5] == 0
     _assert_equal_to_single_calls(ctx, K, poses, pts, pairs, mq, mt, off, out)
-    # n_keep = NULL: the same X and keep
-    img_off = np.r_[0, np.cumsum([len(p) for p in pts])]
-    X, keep, nk = _raw(ctx, K, np.stack([np.stack(p) for p in poses]), pts, img_off, pairs, mq, mt, off, with_nkeep=False)
-    assert nk is None
-    np.testing.assert_array_equal(X, out[0]); np.testing.assert_array_equal(keep, out[1])
-    # only pairs without matches; no pairs at all
+    # only pairs without matches; no pairs at all (n_keep = NULL and the C call without pairs: test_gpu_pair_batch.py)
     X, keep, nk = ctx.triangulate_pairs(K, poses[:2], pts, pairs[:1] * 2, np.zeros(0), np.zeros(0), [0, 0, 0])
     assert X.shape == (0, 3) and keep.shape == (0,) and list(nk) == [0, 0]
     X, keep, nk = ctx.triangulate_pairs(K, np.zeros((0, 2, 3, 4)), pts, np.zeros((0, 2)), np.zeros(0), np.zeros(0), [0])
     assert X.shape == (0, 3) and nk.shape == (0,)
-    _, _, nk = _raw(ctx, K, np.zeros((0, 24)), pts, img_off, np.zeros((0, 2)), np.zeros(0), np.zeros(0), [0])
-    assert nk.shape == (0,)
 
 
 def test_invalid_inputs_are_refused_and_the_context_stays_usable(ctx, cfg1):
+    """through the binding: its own shape checks, and a refusal of the C call; the full table of the C call's refusals is in
+    test_gpu_pair_batch.py"""
     K, Pl, Pr, a, b = _two_views(cfg1)
     idx = np.arange(60)
-    pose = np.stack([Pl, Pr]).reshape(1, 24)
-    good = dict(img_off=[0, len(a), len(a) + len(b)], pairs=[(0, 1)], mq=idx, mt=idx, moff=[0, 60])
-    ref = _raw(ctx, K, pose, [a, b], **good)
+    good = dict(K=K, poses=[(Pl, Pr)], points=[a, b], pairs=[(0, 1)], match_q=idx, match_t=idx, match_off=[0, 60])
+    ref = ctx.triangulate_pairs(**good)
     X1, keep1, nk1 = ctx.triangulate(K, Pl, Pr, a, b, idx, idx)
-    np.testing.assert_array_equal(ref[0], X1); assert ref[2][0] == nk1
-    bad = [(dict(pairs=[(0, 2)]), "outside \\[0, 2\\)"),
-           (dict(pairs=[(-1, 1)]), "outside \\[0, 2\\)"),
-           (dict(img_off=[0, len(a) + 10, len(a)]), "img_off is not monotone"),
-           (dict(img_off=[1, len(a), len(a) + len(b)]), "img_off\\[0\\] must be 0"),
-           (dict(pairs=[(0, 1), (0, 1)], moff=[0, 60, 30]), "match_off is not monotone"),
-           (dict(moff=[5, 60]), "match_off\\[0\\] must be 0"),
-           (dict(mq=np.r_[idx[:59], len(a)]), "indexes outside its images"),
-           (dict(mt=np.r_[-1, idx[1:]]), "indexes outside its images")]
-    for change, msg in bad:
-        args = {**good, **change}
-        poses = np.repeat(pose, len(args["pairs"]), 0)
-        with pytest.raises(capi.SfmB200Error, match=msg):
-            _raw(ctx, K, poses, [a, b], **args)
-        again = _raw(ctx, K, pose, [a, b], **good)
-        for x, y in zip(again, ref):
+    np.testing.assert_array_equal(ref[0], X1); np.testing.assert_array_equal(ref[1], keep1); assert ref[2][0] == nk1
+    bad = [(dict(poses=[(Pl, Pr)] * 2), ValueError, "one \\(Pleft, Pright\\) per pair"),
+           (dict(match_off=[0, 59]), ValueError, "match_off must have"),
+           (dict(pairs=[(0, 2)]), capi.SfmB200Error, "outside \\[0, 2\\)"),
+           (dict(match_q=np.r_[idx[:59], len(a)]), capi.SfmB200Error, "indexes outside its images")]
+    for change, err, msg in bad:
+        with pytest.raises(err, match=msg):
+            ctx.triangulate_pairs(**{**good, **change})
+        for x, y in zip(ctx.triangulate_pairs(**good), ref):
             np.testing.assert_array_equal(x, y)
 
 

@@ -198,6 +198,7 @@ def measure_essential(ctx, reps=20, profile=False):
     50-image set (1225 pairs) in one call, and with profile=True the per-kernel device time of each from torch.profiler in a
     separate pass."""
     import cv2
+    from sfm_toy_library_b200 import capi
     g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
     K = np.array([[2500, 0, 512], [0, 2500, 384], [0, 0, 1]], np.float32)
     pairs = []
@@ -226,9 +227,7 @@ def measure_essential(ctx, reps=20, profile=False):
 
     feats = [g[f"pts_{i}"] for i in range(len(g["files"]))]
     ch_pairs = np.array(g["pairs"], np.int32)
-    ch_q = [g[f"match_{p}_q"] for p in range(len(ch_pairs))]; ch_t = [g[f"match_{p}_t"] for p in range(len(ch_pairs))]
-    ch_off = np.zeros(len(ch_pairs) + 1, np.int64); ch_off[1:] = np.cumsum([len(q) for q in ch_q])
-    ch_q = np.concatenate(ch_q); ch_t = np.concatenate(ch_t)
+    ch_q, ch_t, ch_off = capi.flatten_matches([g[f"match_{p}_q"] for p in range(len(ch_pairs))], [g[f"match_{p}_t"] for p in range(len(ch_pairs))])
     sy = synthetic_essential_set()
 
     def timed(fn, n):
@@ -286,12 +285,11 @@ def measure_homography(ctx, images=50, reps=3):
     kernel time of the batched calls from torch.profiler in a separate pass."""
     import cv2
     import torch
+    from sfm_toy_library_b200 import capi
     g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
     feats = [g[f"pts_{i}"] for i in range(len(g["files"]))]
     ch_pairs = np.array(g["pairs"], np.int32)
-    ch_q = [g[f"match_{p}_q"] for p in range(len(ch_pairs))]; ch_t = [g[f"match_{p}_t"] for p in range(len(ch_pairs))]
-    ch_off = np.zeros(len(ch_pairs) + 1, np.int64); ch_off[1:] = np.cumsum([len(q) for q in ch_q])
-    ch_q = np.concatenate(ch_q); ch_t = np.concatenate(ch_t)
+    ch_q, ch_t, ch_off = capi.flatten_matches([g[f"match_{p}_q"] for p in range(len(ch_pairs))], [g[f"match_{p}_t"] for p in range(len(ch_pairs))])
     sy = synthetic_homography_set(images)
 
     def timed(fn):
@@ -344,7 +342,7 @@ def measure_triangulate_pairs(ctx, reps=20, profile=False):
     separate pass."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     from cfg1_util import Cfg1
-    from sfm_toy_library_b200 import synth
+    from sfm_toy_library_b200 import capi, synth
     cfg1 = Cfg1()
     pts = [f.points for f in cfg1.features]
     loops = {}
@@ -354,9 +352,8 @@ def measure_triangulate_pairs(ctx, reps=20, profile=False):
     ch_single = [(c["K"], c["Pl"], c["Pr"], pts[int(c["pair"][0])], pts[int(c["pair"][1])], c["mq"], c["mt"]) for lp in loops for c in lp]
     ch_batch = []
     for lp in loops:
-        off = np.zeros(len(lp) + 1, np.int64); off[1:] = np.cumsum([len(c["mq"]) for c in lp])
         ch_batch.append((lp[0]["K"], [(c["Pl"], c["Pr"]) for c in lp], pts, [tuple(int(x) for x in c["pair"]) for c in lp],
-                         np.concatenate([c["mq"] for c in lp]), np.concatenate([c["mt"] for c in lp]), off))
+                         *capi.flatten_matches([c["mq"] for c in lp], [c["mt"] for c in lp])))
     K, poses, spts, spairs, smq, smt, soff = sy = synth.make_triangulation_pairs(50, seed=0)
     sy_single = [(K, poses[p][0], poses[p][1], spts[i], spts[j], smq[soff[p]:soff[p + 1]], smt[soff[p]:soff[p + 1]]) for p, (i, j) in enumerate(spairs)]
     arms = {"crazyhorse_20_single_calls": lambda: [ctx.triangulate(*a) for a in ch_single],
