@@ -197,7 +197,13 @@ void sfmb200_ba_default_options(sfmb200_ba_options* opt);
 /* Host-only check of a flattened problem: CSR offsets monotone from 0 to nobs, cameras in [0, nc) and strictly ascending
  * inside a point (the std::map order of reference :146), at most 255 views per point.  sfmb200_ba_problem_create /
  * sfmb200_ba_solve run the same check; exported so that a host can validate without a device.  0 = valid; otherwise
- * SFMB200_ERR_INVALID / _UNSUPPORTED with the reason in `message`. */
+ * SFMB200_ERR_INVALID / _UNSUPPORTED with the reason in `message`.
+ * A problem this accepts is also accepted by sfmb200_ba_problem_create in the default (gather) Schur mode.  The atomics
+ * ("red") Schur mode keeps a point's Schur terms in shared memory and supports at most 244 views per point: create refuses
+ * more with SFMB200_ERR_UNSUPPORTED and "observations per point (k) exceed the shared-memory budget of the atomics ("red")
+ * Schur mode".  That mode runs with SFMB200_BA_SCHUR=red, and create chooses it by itself for large problems whose pair
+ * lists outgrow the gather mode's buffers: thousands of cameras, 2^31 - 1024 or more pairs of observations of one point summed
+ * over the points, or per-camera-pair partial blocks beyond 256 MB. */
 int sfmb200_ba_validate(int nc, int np, int nobs, const int32_t* obs_cam, const int32_t* pt_off, char* message, int message_len);
 
 /*

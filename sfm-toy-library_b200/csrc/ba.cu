@@ -1163,7 +1163,7 @@ template <int G> static int launch_backsub(sfmb200_ba_problem* P, const BAView& 
     sfmb200_ctx* ctx = P->ctx;
     const int GB = PT_THREADS / G, nxt = P->cur ^ 1;
     if (P->backsub_from_z) {            // gather mode: Z_o is in Zbuf, no Jacobian needed (inside the LM loop the radius comes from LMState)
-        const size_t tab = sizeof(double) * 18 * (size_t)P->nc;
+        const size_t tab = sizeof(double) * 18 * (size_t)P->nc;     // (above 212 cameras opted in by create)
         if (tab <= 40 * 1024) {
             const int blocks = resident_grid(P, &P->grid_backsub, ba_backsub_z_kernel<G, true>, PT_THREADS, tab, ceil_div(P->np, GB));
             ba_backsub_z_kernel<G, true><<<blocks, PT_THREADS, tab, ctx->stream>>>(v, 0.0, P->y_cf, P->cf[nxt], P->camd[nxt], P->pts[nxt], P->post);
@@ -1452,7 +1452,6 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         if (vrc == SFMB200_OK) {
             P->maxk = std::max(maxk, 1);
             P->G = maxk <= 4 ? 4 : maxk <= 8 ? 8 : maxk <= 16 ? 16 : 32;
-            if (point_smem_bytes(P->G, P->maxk) > 200 * 1024) { snprintf(msg, sizeof msg, "observations per point (%d) exceed the shared-memory budget", maxk); vrc = SFMB200_ERR_UNSUPPORTED; }
         }
         if (vrc != SFMB200_OK) { cudaStreamSynchronize(st); ba_release_buffers(P); delete P; return sfmb200_fail(ctx, vrc, "%s", msg); }
     }
@@ -1483,6 +1482,12 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         const size_t nseg_est = (size_t)pair_segments(ctx, nobs);
         const bool partials_fit = nblk * nseg_est * 288 <= ((size_t)256 << 20);
         P->gather = !(mode && strcmp(mode, "red") == 0) && (size_t)(2 * PFILL_WARPS + 1) * nc * 4 <= 160 * 1024 && pair_entries < (1LL << 31) - 1024 && partials_fit;
+        // only the "red" point kernel stages a point's Z blocks in shared memory (gather mode launches it without dynamic
+        // shared memory): with G = 32 that is maxk^2 + 591 maxk + 16 bytes, so a point with more than 244 views is refused here
+        if (!P->gather && point_smem_bytes(P->G, P->maxk) > 200 * 1024) {
+            cudaStreamSynchronize(st); ba_release_buffers(P); delete P;
+            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "observations per point (%d) exceed the shared-memory budget of the atomics (\"red\") Schur mode", maxk);
+        }
     }
     if (nobs) {
         expand_obs_pt_kernel<<<ceil_div(np, 256), 256, 0, st>>>(P->pt_off, np, obs_pt);
@@ -1572,6 +1577,16 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         // that would come from HBM.  SFMB200_BA_BACKSUB=stored / jacobian forces either.
         const bool z_in_l2 = P->pair_nseg == 1;
         P->backsub_from_z = P->gather && P->Zbuf && (bm ? strcmp(bm, "stored") == 0 : z_in_l2);
+        // ba_backsub_z_kernel stages the camera table (144 B per camera, up to 40 KB) next to 18.1 KB of static shared memory
+        // (zstage, sred): above 212 cameras that passes the 48 KB a launch gets without opting in
+        const size_t tab = sizeof(double) * 18 * (size_t)nc, zstatic = sizeof(double) * (PT_THREADS / 32) * (32 * 18 + 4);
+        if (P->backsub_from_z && tab <= 40 * 1024 && tab + zstatic > 48 * 1024) {
+            const int t = (int)tab;
+            CRT(P->G == 4 ? cudaFuncSetAttribute(ba_backsub_z_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
+                : P->G == 8 ? cudaFuncSetAttribute(ba_backsub_z_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
+                : P->G == 16 ? cudaFuncSetAttribute(ba_backsub_z_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
+                : cudaFuncSetAttribute(ba_backsub_z_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t));
+        }
     }
 #undef CRT
     *out = P;
