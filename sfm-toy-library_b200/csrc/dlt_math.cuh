@@ -1,8 +1,16 @@
 // dlt_math.cuh -- smallest right singular vector of the 4 x 4 two-view DLT matrix (cv::triangulatePoints), shared by the
 // triangulation stage (triangulate.cu) and the cheirality test of the pose recovery (essential.cu).
+// __host__ __device__, so that tests/ can run the very same code on the CPU against an exact reference.
 #pragma once
 #include <cfloat>
 #include <cmath>
+
+#if defined(__CUDACC__)
+#define DLT_HD __host__ __device__ __forceinline__
+#else
+#define DLT_HD inline
+using std::isfinite;   // <cmath> declares the others in the global namespace too
+#endif
 
 namespace {
 
@@ -27,7 +35,7 @@ namespace {
         }                                                                                                         \
     }
 
-__device__ __forceinline__ void null_vector_4x4(double A[4][4], double X[4]) {
+DLT_HD void null_vector_4x4(double A[4][4], double X[4]) {
     double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
     double nrm[4];
 #pragma unroll
@@ -61,12 +69,12 @@ __device__ __forceinline__ void null_vector_4x4(double A[4][4], double X[4]) {
 // column of the adjugate is a multiple of the null vector; the column with the largest diagonal cofactor is used).
 // ~600 flops instead of ~5000 for the Jacobi SVD.  The result is verified (residual of the eigen-equation); anything
 // suspicious falls back to the Jacobi routine above, which is the reference-faithful algorithm.
-__device__ __forceinline__ double det3(double a, double b, double c, double d, double e, double f, double g, double h, double i) {
+DLT_HD double det3(double a, double b, double c, double d, double e, double f, double g, double h, double i) {
     return a * (e * i - f * h) - b * (d * i - f * g) + c * (d * h - e * g);
 }
 struct Sym4 { double c00, c01, c02, c03, c11, c12, c13, c22, c23, c33; };
 struct Adj4 { double k00, k01, k02, k03, k11, k12, k13, k22, k23, k33; };
-__device__ __forceinline__ void adjugate_sym4(const Sym4& m, Adj4& k) {
+DLT_HD void adjugate_sym4(const Sym4& m, Adj4& k) {
     k.k00 = det3(m.c11, m.c12, m.c13, m.c12, m.c22, m.c23, m.c13, m.c23, m.c33);
     k.k01 = -det3(m.c01, m.c12, m.c13, m.c02, m.c22, m.c23, m.c03, m.c23, m.c33);
     k.k02 = det3(m.c01, m.c11, m.c13, m.c02, m.c12, m.c23, m.c03, m.c13, m.c33);
@@ -78,7 +86,7 @@ __device__ __forceinline__ void adjugate_sym4(const Sym4& m, Adj4& k) {
     k.k23 = -det3(m.c00, m.c01, m.c02, m.c01, m.c11, m.c12, m.c03, m.c13, m.c23);
     k.k33 = det3(m.c00, m.c01, m.c02, m.c01, m.c11, m.c12, m.c02, m.c12, m.c22);
 }
-__device__ __forceinline__ bool null_vector_fast(const double A[4][4], double X[4]) {
+DLT_HD bool null_vector_fast(const double A[4][4], double X[4]) {
     Sym4 B;
     B.c00 = A[0][0] * A[0][0] + A[1][0] * A[1][0] + A[2][0] * A[2][0] + A[3][0] * A[3][0];
     B.c01 = A[0][0] * A[0][1] + A[1][0] * A[1][1] + A[2][0] * A[2][1] + A[3][0] * A[3][1];
