@@ -340,6 +340,61 @@ int sfmb200_find_camera_matrices_pairs(sfmb200_ctx* ctx, const float* K, const f
                                        const int64_t* match_off, const sfmb200_essential_options* opt, double* E, double* R, double* t,
                                        uint8_t* inlier_mask, uint8_t* pose_mask, sfmb200_essential_summary* summary);
 
+/* ---- f-2: camera pose from 2D-3D matches (PnP RANSAC + refit), all on the device ------------------------------ */
+/*
+ * findCameraPoseFrom2D3DMatch (SfMStereoUtilities.cpp:208-243):
+ *     solvePnPRansac(points3D, points2D, K, distortion, rvec, t, false, 100, RANSAC_THRESHOLD = 10, 0.99, inliers)
+ * in one call.  max_iters samples of 5 distinct correspondences are drawn from the generator of the essential-matrix RANSAC
+ * (splitmix64 keyed by seed, sample and draw; a repeated index is redrawn).  Every sample is solved by EPnP in fp64 (at most one
+ * pose; a degenerate sample -- coincident, collinear or coplanar 3D points, a rank-deficient system, a non-finite result -- gives
+ * none).  Every pose is scored with the reprojection error and inlier rule of sfmb200_ransac_score (SFMB200_MODEL_POSE: double
+ * projection, float difference, err <= (float)(threshold_px^2)), and OpenCV's sequential loop (RANSACPointSetRegistrator::run with
+ * model_points = 5) is replayed over the counts in sample order: a pose replaces the best one only if its count exceeds
+ * max(best count, 4), every improvement recomputes the sample budget with RANSACUpdateNumIters(confidence, outlier ratio, 5,
+ * budget), and the loop stops at the budget.  cv:: draws its samples from its own RNG, so the RANSAC agrees with cv:: only
+ * statistically.
+ * Refit: with 6 or more inliers, damped Gauss-Newton (Levenberg-Marquardt) on (angle-axis, t) from the winner's pose minimises the
+ * summed squared pixel reprojection error over the winner's inliers, at most refine_iters iterations, stopping when the relative
+ * step or cost change falls below 1e-10: the least-squares minimum cv::solvePnP(SOLVEPNP_ITERATIVE) reaches on the same inliers.
+ * If the refit does not lower the cost, the RANSAC pose is returned with summary.refined = 0.
+ *   K [9] float row-major: fx = K[0], fy = K[4], cx = K[2], cy = K[5]; no distortion.  pts3 [m*3], pts2 [m*2] float.
+ *   rvec [3] angle-axis, R [9] row-major (R = Rodrigues(rvec)), t [3], double; inlier_mask [m] = the RANSAC winner's inliers
+ *   (solvePnPRansac's `inliers` output, before the refit; summary.n_inliers is their number).  Any output may be NULL.  opt NULL
+ *   = defaults.  A correspondence with a non-finite coordinate is never an inlier.
+ *   m < 5: SFMB200_OK with summary.found = 0 and zero outputs (cv::solvePnPRansac runs P3P at m == 4 and asserts below that).
+ *   m == 5: EPnP on the five points, mask all ones, no refit (solvePnPRansac's model_points == npoints branch); found = 0 when
+ *   the five points are degenerate.
+ *   No pose with more than 4 inliers: found = 0 and zero outputs.
+ *   SFMB200_ERR_INVALID: bad options, a NULL K, NULL points with m > 0, m < 0, a non-finite K entry, fx <= 0 or fy <= 0.
+ * Four launches (solve, score, select, mask + refit), one upload, one download, one host synchronisation per call.  Same seed,
+ * same inputs: bitwise-identical outputs.
+ */
+typedef struct {
+    int max_iters;            /* 100   (SfMStereoUtilities.cpp:225); in [1, 2^24] */
+    double confidence;        /* 0.99  (:225); in (0, 1) */
+    double threshold_px;      /* 10    RANSAC_THRESHOLD (:41); finite, > 0 */
+    int refine_iters;         /* 20    iterations of the refit; 0 = no refit (the RANSAC pose) */
+    uint64_t seed;            /* 0 */
+} sfmb200_pose_options;
+typedef struct {
+    int found;                /* 1: a pose with more than 4 inliers (m == 5: EPnP succeeded) */
+    int n_inliers;            /* inliers of the RANSAC winner (the mask) */
+    int iterations;           /* samples the sequential loop visited */
+    int n_samples;            /* samples drawn and solved */
+    int n_hypotheses;         /* samples that gave a pose */
+    int refined;              /* 1: the returned pose is the refit's */
+} sfmb200_pose_summary;
+void sfmb200_pose_default_options(sfmb200_pose_options* opt);
+int sfmb200_find_camera_pose(sfmb200_ctx* ctx, const float* K, const float* pts3, const float* pts2, int m, const sfmb200_pose_options* opt,
+                             double* rvec, double* R, double* t, uint8_t* inlier_mask, sfmb200_pose_summary* summary);
+/* Test hooks.  sfmb200_epnp: the device minimal solver on ns given samples, X [ns][5][3] world points, uv [ns][5][2] pixels, K [9]
+ * double row-major -> Rt [ns][12] row-major [R|t] (zeros where ok = 0), ok [ns].  The RANSAC runs the same machine code.
+ * sfmb200_pose_last_trace: the last sfmb200_find_camera_pose call's samples [cap][5] and per-sample inlier counts [cap] (-1: the
+ * sample gave no pose), for its first min(cap, n_samples) samples; either output may be NULL.  Returns that call's n_samples (0
+ * before any call or after a call with m < 5), or -1 on bad arguments. */
+int sfmb200_epnp(sfmb200_ctx* ctx, const double* X, const double* uv, const double* K, int ns, double* Rt, uint8_t* ok);
+int sfmb200_pose_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, int32_t* counts);
+
 /* ---- f-2: homography RANSAC for many image pairs, all on the device -------------------------------------------- */
 /*
  * findHomographyInliers (SfMStereoUtilities.cpp:51-72) for every pair of a batch in one call:

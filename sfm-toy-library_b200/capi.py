@@ -61,6 +61,19 @@ class EssentialSummary(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class PoseOptions(C.Structure):
+    _fields_ = [("max_iters", C.c_int), ("confidence", C.c_double), ("threshold_px", C.c_double), ("refine_iters", C.c_int),
+                ("seed", C.c_uint64)]
+
+
+class PoseSummary(C.Structure):
+    _fields_ = [("found", C.c_int), ("n_inliers", C.c_int), ("iterations", C.c_int), ("n_samples", C.c_int), ("n_hypotheses", C.c_int),
+                ("refined", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class HomographyOptions(C.Structure):
     _fields_ = [("max_iters", C.c_int), ("confidence", C.c_double), ("threshold_px", C.c_double), ("refine_iters", C.c_int),
                 ("record_trace", C.c_int)]
@@ -323,6 +336,43 @@ class Context:
             raise SfmB200Error("sfmb200_essential_last_trace failed")
         return smp[:S], n[:S], c[:int(n[:S].sum())]
 
+    # ------------------------------------------------------------------ f-2 PnP RANSAC + refit
+    def find_camera_pose(self, K, pts3, pts2, options=None, **kw):
+        """sfmb200_find_camera_pose: cv::solvePnPRansac's job on the device (seeded EPnP samples, OpenCV's selection, least-squares
+        refit).  pts3 [m, 3], pts2 [m, 2] float; options: PoseOptions or keyword overrides of the defaults (max_iters, confidence,
+        threshold_px, refine_iters, seed).  Returns (rvec [3], R [3, 3], t [3], inlier_mask [m], summary dict)."""
+        K = np.ascontiguousarray(K, np.float32).reshape(9)
+        X = np.ascontiguousarray(pts3, np.float32).reshape(-1, 3); uv = np.ascontiguousarray(pts2, np.float32).reshape(-1, 2)
+        if X.shape[0] != uv.shape[0]:
+            raise ValueError("find_camera_pose: as many 3D as 2D points")
+        m = X.shape[0]
+        o = options or pose_default_options(**kw)
+        rv = np.zeros(3); Rm = np.zeros(9); t = np.zeros(3); mask = np.zeros(max(m, 1), np.uint8); s = PoseSummary()
+        self._check(lib().sfmb200_find_camera_pose(self._h, _p(K, C.c_float), _p(X, C.c_float), _p(uv, C.c_float), m, C.byref(o), _p(rv, C.c_double),
+                                                   _p(Rm, C.c_double), _p(t, C.c_double), _p(mask, C.c_uint8), C.byref(s)))
+        return rv, Rm.reshape(3, 3), t, mask[:m], s.as_dict()
+
+    def epnp(self, X, uv, K):
+        """sfmb200_epnp: the device EPnP solver on given samples, X [ns, 5, 3], uv [ns, 5, 2] pixels, K [3, 3] ->
+        (Rt [ns, 3, 4], ok [ns])."""
+        X = np.ascontiguousarray(X, np.float64).reshape(-1, 5, 3); uv = np.ascontiguousarray(uv, np.float64).reshape(-1, 5, 2)
+        K = np.ascontiguousarray(K, np.float64).reshape(9)
+        ns = X.shape[0]
+        Rt = np.zeros((max(ns, 1), 12)); ok = np.zeros(max(ns, 1), np.uint8)
+        self._check(lib().sfmb200_epnp(self._h, _p(X, C.c_double), _p(uv, C.c_double), _p(K, C.c_double), ns, _p(Rt, C.c_double), _p(ok, C.c_uint8)))
+        return Rt[:ns].reshape(ns, 3, 4), ok[:ns]
+
+    def pose_last_trace(self):
+        """sfmb200_pose_last_trace: (samples [S, 5], inlier counts [S], -1 where a sample gave no pose) of the last find_camera_pose."""
+        f = lib().sfmb200_pose_last_trace
+        S = f(self._h, 0, None, None)
+        if S < 0:
+            raise SfmB200Error("sfmb200_pose_last_trace failed")
+        smp = np.zeros((max(S, 1), 5), np.int32); c = np.zeros(max(S, 1), np.int32)
+        if f(self._h, S, _p(smp, C.c_int32), _p(c, C.c_int32)) != S:
+            raise SfmB200Error("sfmb200_pose_last_trace failed")
+        return smp[:S], c[:S]
+
     # ------------------------------------------------------------------ f-2 homography RANSAC for many pairs
     def find_homography_pairs(self, points, pairs, match_q, match_t, match_off, options=None, **kw):
         """sfmb200_find_homography_pairs: cv::findHomography(RANSAC) for every pair in one call.  points: list of [n_i, 2] key
@@ -542,6 +592,14 @@ def ba_default_options(**kw):
 def essential_default_options(**kw):
     o = EssentialOptions()
     lib().sfmb200_essential_default_options(C.byref(o))
+    for k, v in kw.items():
+        setattr(o, k, v)
+    return o
+
+
+def pose_default_options(**kw):
+    o = PoseOptions()
+    lib().sfmb200_pose_default_options(C.byref(o))
     for k, v in kw.items():
         setattr(o, k, v)
     return o

@@ -153,26 +153,21 @@ essential_select_kernel(const EsPair* __restrict__ pr, int np, const int32_t* __
     const EsPair P = pr[p];
     const int32_t* ns = nsol + P.s0;
     const int32_t* cs = counts + 10 * (size_t)P.s0;
-    int niters = max(max_iters, 1), best = -1, max_good = 0, iter = 0, nh = 0;
+    SeqSelect st;
+    seq_select_begin(st, max_iters);
+    int nh = 0;
     for (int base = 0; base < P.S; base += 32) {
         const int k = min(32, P.S - base);
         const int v = lane < k ? ns[base + lane] : 0;
         nh += v;
-        if (!__shfl_sync(0xffffffffu, iter < niters, 0)) continue;    // the loop has stopped: only the solution total is left
+        if (!__shfl_sync(0xffffffffu, st.iter < st.niters, 0)) continue;    // the loop has stopped: only the solution total is left
         sn[w][lane] = v;
         for (int q = lane; q < 10 * k; q += 32) sc[w][q] = cs[10 * (size_t)base + q];
         __syncwarp();
-        if (lane == 0)
-            for (int j = 0; j < k && iter < niters; ++j, ++iter)
-                for (int q = 0; q < sn[w][j]; ++q) {
-                    const int g = sc[w][10 * j + q];
-                    if (g > max(max_good, 4)) {
-                        best = 10 * (P.s0 + iter) + q; max_good = g;
-                        niters = ransac_update_num_iters(confidence, (double)(P.m - g) / P.m, 5, niters);
-                    }
-                }
+        if (lane == 0) seq_select_chunk(st, sn[w], sc[w], 10, k, P.m, confidence, 5, 10 * P.s0);
         __syncwarp();
     }
+    const int best = st.best, max_good = st.max_good, iter = st.iter;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) nh += __shfl_xor_sync(0xffffffffu, nh, o);
     if (lane != 0) return;

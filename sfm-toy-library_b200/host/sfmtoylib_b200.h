@@ -38,6 +38,8 @@ public:
     static Matching matchFeatures(const Features& featuresLeft, const Features& featuresRight);
 };
 
+struct Image2D3DMatch;        // sfm_glue.h (SfMCommon.h:71-74)
+
 class SfMStereoUtilities {
 public:
     static int findHomographyInliers(const Features& left, const Features& right, const Matching& matches);
@@ -46,6 +48,7 @@ public:
     static bool triangulateViews(const Intrinsics& intrinsics, const ImagePair imagePair, const Matching& matches,
                                  const Features& featuresLeft, const Features& featuresRight, const cv::Matx34f& Pleft,
                                  const cv::Matx34f& Pright, PointCloud& pointCloud);
+    static bool findCameraPoseFrom2D3DMatch(const Intrinsics& intrinsics, const Image2D3DMatch& match, cv::Matx34f& cameraPose);
 };
 
 class SfMBundleAdjustmentUtils {

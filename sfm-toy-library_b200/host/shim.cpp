@@ -10,6 +10,9 @@
 #include "SfMToyLib/SfMBundleAdjustmentUtils.h"
 #else
 #include "sfmtoylib_b200.h"
+#ifdef SFMB200_SHIM_POSE
+#include "sfm_glue.h"
+#endif
 #endif
 #include "../../include/sfmb200.h"
 
@@ -51,6 +54,9 @@ const int kType8U = cv::CV_8U;                // cv_min.h
 #endif
 const double kNNMatchRatio = 0.8f;            // NN_MATCH_RATIO: the float literal widened to double
 const float kMaxReprojectionError = 10.0f;    // MIN_REPROJECTION_ERROR
+#if defined(SFMB200_SHIM_POSE) && !defined(SFMB200_WITH_REFERENCE_HEADERS)
+const float POSE_INLIERS_MINIMAL_RATIO = 0.5f;   // SfMCommon.h:53
+#endif
 
 }  // namespace
 
@@ -196,6 +202,39 @@ int SfMStereoUtilities::findHomographyInliers(const Features& left, const Featur
     return summary.found ? summary.n_inliers : 0;
 }
 #endif  // SFMB200_SHIM_HOMOGRAPHY
+
+#ifdef SFMB200_SHIM_POSE           // define it to replace findCameraPoseFrom2D3DMatch (OpenCV's solvePnPRansac) too
+// SfMStereoUtilities.cpp:208-243: PnP RANSAC and the least-squares refit in one device call (sfmb200_find_camera_pose, 100 samples,
+// RANSAC_THRESHOLD, 0.99), then the reference's inlier-ratio test on the RANSAC inlier count; cameraPose is written only when the
+// pose is accepted.
+bool SfMStereoUtilities::findCameraPoseFrom2D3DMatch(const Intrinsics& intrinsics, const Image2D3DMatch& match, cv::Matx34f& cameraPose) {
+    const int m = (int)match.points2D.size();
+    if ((int)match.points3D.size() != m) {
+        std::cerr << "findCameraPoseFrom2D3DMatch: " << match.points3D.size() << " 3D points for " << m << " 2D points" << std::endl;
+        return false;
+    }
+    float K[9];
+    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) K[3 * r + c] = intrinsics.K.at<float>(r, c);
+    static_assert(sizeof(cv::Point3f) == 3 * sizeof(float), "Point3f must be three packed floats");
+    sfmb200_pose_options opt;
+    sfmb200_pose_default_options(&opt);                                                 // 100 iterations, 10 px, 0.99 (:225)
+    double R[9], t[3];
+    sfmb200_pose_summary summary;
+    check(sfmb200_find_camera_pose(context(), K, reinterpret_cast<const float*>(match.points3D.data()),
+                                   reinterpret_cast<const float*>(match.points2D.data()), m, &opt, nullptr, R, t, nullptr, &summary),
+          "sfmb200_find_camera_pose");
+    const int n_in = summary.found ? summary.n_inliers : 0;
+    if ((float)n_in / (float)m < POSE_INLIERS_MINIMAL_RATIO) {                         // :231-234
+        std::cerr << "Inliers ratio is too small: " << n_in << " / " << m << std::endl;
+        return false;
+    }
+    for (int r = 0; r < 3; ++r) {                                                       // :236-240
+        for (int c = 0; c < 3; ++c) cameraPose(r, c) = (float)R[3 * r + c];
+        cameraPose(r, 3) = (float)t[r];
+    }
+    return true;
+}
+#endif  // SFMB200_SHIM_POSE
 
 void SfMBundleAdjustmentUtils::adjustBundle(PointCloud& pointCloud, std::vector<Pose>& cameraPoses, Intrinsics& intrinsics,
                                             const std::vector<Features>& image2dFeatures) {

@@ -168,3 +168,16 @@ def findCameraPoseFrom2D3DMatch(intrinsics: Intrinsics, points2D, points3D, ctx=
         if ok:
             R, _ = cv2.Rodrigues(rvec); P = np.concatenate([R, tvec.reshape(3, 1)], 1)
     return True, P.astype(np.float32)
+
+
+def findCameraPoseFrom2D3DMatch_gpu(intrinsics: Intrinsics, points2D, points3D, ctx=None, seed=0):
+    """SfMStereoUtilities::findCameraPoseFrom2D3DMatch (SfMStereoUtilities.cpp:208-243) entirely on the device
+    (sfmb200_find_camera_pose: seeded EPnP samples, OpenCV's sequential selection, least-squares refit on the winner's inliers), then
+    the reference's float inlier-ratio test on the RANSAC inlier count.  Returns (success, pose 3x4 float32) like the reference."""
+    ctx = ctx or default_context()
+    _, R, t, _, s = ctx.find_camera_pose(intrinsics.K, points3D, points2D, seed=seed, threshold_px=RANSAC_THRESHOLD)
+    if not s["found"]:
+        return False, None
+    if np.float32(s["n_inliers"]) / np.float32(len(points2D)) < np.float32(POSE_INLIERS_MINIMAL_RATIO):     # :231-234
+        return False, None
+    return True, np.concatenate([R, t.reshape(3, 1)], 1).astype(np.float32)                                # :236-240

@@ -395,6 +395,77 @@ def measure_triangulate_pairs(ctx, reps=20, profile=False):
     return out
 
 
+POSE_KERNELS = ("pose_solve_kernel", "pose_score_kernel", "pose_select_kernel", "pose_refit_kernel")
+
+
+def pose_kernel_ms(fn):
+    """device time per K9 kernel (ms, summed over its launches) of one fn() under torch.profiler"""
+    import torch
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    out = {k: 0.0 for k in POSE_KERNELS}
+    for e in prof.events():
+        for k in POSE_KERNELS:
+            if k in e.name:
+                out[k] += 1e-3 * e.device_time_total
+    out["total"] = sum(out.values())
+    return out
+
+
+def measure_pose(ctx, reps=20, profile=False):
+    """findCameraPoseFrom2D3DMatch (SfMStereoUtilities.cpp:208-243) on the five PnP sets of the crazyhorse replay
+    (tests/golden/cfg1_crazyhorse.npz, with the intrinsics of each call): sfmb200_find_camera_pose (host clock around the synchronised
+    call, warmed up, median over reps per set) against cv2.solvePnPRansac(100, 10 px, 0.99) on one thread and on all threads; a
+    seeded synthetic set of 100 000 correspondences with 30 % outliers; with profile=True the per-kernel device time from
+    torch.profiler in a separate pass."""
+    import cv2
+    g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
+    sets = [(g[f"pnp_{k}_p3"], g[f"pnp_{k}_p2"], np.asarray(g[f"ba_{k}_K_after"], np.float32)) for k in range(int(g["n_pnp"]))]
+    rs = np.random.RandomState(0)
+    n = 100_000
+    Ks = np.array([[1200, 0, 640], [0, 1150, 360], [0, 0, 1]], np.float32)
+    Xc = np.c_[rs.uniform(-3, 3, (n, 2)), rs.uniform(4, 12, n)]
+    uv = Xc[:, :2] / Xc[:, 2:] * [1200, 1150] + [640, 360] + rs.normal(0, 0.5, (n, 2))
+    bad = rs.uniform(size=n) < 0.3
+    uv[bad] = rs.uniform([0, 0], [1280, 720], (int(bad.sum()), 2))
+    syn = (Xc.astype(np.float32), uv.astype(np.float32), Ks)
+
+    def timed(X, p2, K, r):
+        ctx.find_camera_pose(K, X, p2)
+        ts = []
+        for _ in range(r):
+            t0 = time.perf_counter(); ctx.find_camera_pose(K, X, p2); ts.append(1e3 * (time.perf_counter() - t0))
+        return ts
+    gpu = [float(np.median(timed(X, p2, K, reps))) for X, p2, K in sets]
+    t_syn = timed(*syn, 5)
+
+    def cv_ms(threads, data, r=5):
+        cv2.setNumThreads(threads)
+        out = []
+        for X, p2, K in data:
+            ts = []
+            for _ in range(r):
+                t0 = time.perf_counter()
+                cv2.solvePnPRansac(X.reshape(-1, 1, 3), p2.reshape(-1, 1, 2), K, np.zeros((1, 4), np.float32), None, None, False, 100, 10.0, 0.99)
+                ts.append(1e3 * (time.perf_counter() - t0))
+            out.append(float(np.median(ts)))
+        return out
+    one = cv_ms(1, sets); allt = cv_ms(os.cpu_count() or 1, sets)
+    syn_one = cv_ms(1, [syn], 1)[0]; syn_all = cv_ms(os.cpu_count() or 1, [syn], 1)[0]
+    cv2.setNumThreads(-1)
+    kernels = {"crazyhorse_%d" % k: pose_kernel_ms(lambda X=X, p2=p2, K=K: ctx.find_camera_pose(K, X, p2)) for k, (X, p2, K) in enumerate(sets)}
+    if profile:
+        kernels["synthetic_100000"] = pose_kernel_ms(lambda: ctx.find_camera_pose(syn[2], syn[0], syn[1]))
+    name, pl = card()
+    return {"metric": "pnp_ransac_pose_ms_per_call", "gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt,
+            "correspondences": [int(len(X)) for X, _, _ in sets], "gpu_median_ms": float(np.median(gpu)),
+            "cv2_1thread_median_ms": float(np.median(one)), "cv2_all_threads_median_ms": float(np.median(allt)),
+            "synthetic_100000_gpu_median_ms": float(np.median(t_syn)), "synthetic_100000_cv2_1thread_ms": syn_one,
+            "synthetic_100000_cv2_all_threads_ms": syn_all, "kernel_ms_torch_profiler": kernels if profile else "not profiled",
+            "card": name, "power_limit": pl, "cpu_threads": os.cpu_count()}
+
+
 def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, stages=("match", "triangulate", "essential"), profile=False):
     import torch
     from sfm_toy_library_b200 import capi
@@ -414,6 +485,8 @@ def measure_all(images=50, features=5000, points=1_000_000, reps=5, ctx=None, st
         out.append(measure_homography(ctx, images))
     if "triangulate-pairs" in stages:
         out.append(measure_triangulate_pairs(ctx, profile=profile))
+    if "pose" in stages:
+        out.append(measure_pose(ctx, profile=profile))
     if own:
         ctx.close()
     return out
@@ -425,8 +498,8 @@ def main():
     ap.add_argument("--features", type=int, default=5000)
     ap.add_argument("--points", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography, triangulate-pairs")
-    ap.add_argument("--no-profile", action="store_true", help="skip the torch.profiler kernel split of the essential and triangulate-pairs stages")
+    ap.add_argument("--stages", default="match,triangulate,essential", help="comma-separated subset of match, triangulate, essential, homography, triangulate-pairs, pose")
+    ap.add_argument("--no-profile", action="store_true", help="skip the torch.profiler kernel split of the essential, triangulate-pairs and pose stages")
     args = ap.parse_args()
     for line in measure_all(args.images, args.features, args.points, args.reps, stages=args.stages.split(","), profile=not args.no_profile):
         print(json.dumps(line), flush=True)
