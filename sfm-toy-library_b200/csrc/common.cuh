@@ -13,6 +13,7 @@
 
 #include "../../include/sfmb200.h"
 #include "host_pool.h"
+#include "match_cache.h"
 
 // One growable device buffer + one pinned host buffer per purpose, reused across calls (cudaMalloc/cudaFree are
 // milliseconds; the reference calls each stage many times per runSfM()).
@@ -67,16 +68,10 @@ struct BAWorkspace {
 };
 
 // Descriptor images kept resident between per-call matchFeatures invocations (match.cu): one arena of packed rows, one of
-// expanded tensor-core operand blocks, bump-allocated, flushed whole when full.
-struct MatchCacheEntry { const void* host; int rows; int desc_bytes; uint64_t hash; int row0; int blk0; };
-struct MatchCache {
+// expanded tensor-core operand blocks, bump-allocated, flushed whole when full (bookkeeping and capacity plan: match_cache.h).
+struct MatchCache : MatchCacheState {
     DevBuf desc, exp;
-    int width = 0;                       // padded descriptor width (bytes) of the rows in the arena
-    int64_t rows_cap = 0, rows_used = 0;
-    int blk_cap = 0, blk_used = 0;
-    std::vector<MatchCacheEntry> entries;
-    int64_t hits = 0, misses = 0;
-    void release() { desc.release(); exp.release(); entries.clear(); rows_cap = rows_used = 0; blk_cap = blk_used = 0; }
+    void release() { desc.release(); exp.release(); reset(); }
 };
 
 // Device buffers of the last ORB extraction (orb.cu), kept for sfmb200_orb_download_level (stage-by-stage parity tests).

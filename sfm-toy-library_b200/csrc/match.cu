@@ -549,15 +549,24 @@ static uint64_t content_hash(const uint8_t* p, size_t n) {
     return h0 ^ (h1 * 3) ^ (h2 * 5) ^ (h3 * 7) ^ (uint64_t)n;
 }
 
-// make `img` (rows x desc_bytes host bytes) resident; returns its first row / first expanded block in the arena
+// make `img` (rows x desc_bytes host bytes) resident; returns its first row / first expanded block in the arena.
+// Capacity rule: match_cache_plan keeps rows_cap * width + 16 <= desc.cap and blk_cap * block bytes <= exp.cap after every call,
+// recomputing rows_cap from desc.cap whenever the padded width changes (a buffer sized for 16-byte rows holds an eighth as many
+// 128-byte rows).  The plan flushes or grows the arena until the call's new images fit under rows_cap / blk_cap; the check below
+// holds every placement to the buffers themselves, so a planning mistake is an error status, never a copy past an allocation.
 static int cache_acquire(sfmb200_ctx* ctx, const uint8_t* img, int rows, int desc_bytes, int width, uint64_t hash, int& row0, int& blk0) {
     MatchCache& mc = ctx->mcache;
-    for (const MatchCacheEntry& e : mc.entries)
-        if (e.host == img && e.rows == rows && e.desc_bytes == desc_bytes && e.hash == hash) { row0 = e.row0; blk0 = e.blk0; mc.hits++; return SFMB200_OK; }
+    if (const MatchCacheEntry* e = mc.find(img, rows, desc_bytes, hash)) { row0 = e->row0; blk0 = e->blk0; mc.hits++; return SFMB200_OK; }
     mc.misses++;
     const int br = match_tc_block_rows();
     const int nblk = width == 32 ? ceil_div(rows, br) : 0;
     row0 = (int)mc.rows_used; blk0 = mc.blk_used;
+    if (!match_cache_fits(mc, rows, nblk, width, match_tc_block_bytes(false), mc.desc.cap, mc.exp.cap)) {
+        const int64_t used = mc.rows_used;
+        mc.reset();
+        return sfmb200_fail(ctx, SFMB200_ERR_NOMEM, "per-call matcher arena: %d rows of %d bytes at row %lld (+%d blocks at block %d) exceed its "
+                            "buffers (%zu / %zu bytes); the arena was cleared", rows, width, (long long)used, nblk, blk0, mc.desc.cap, mc.exp.cap);
+    }
     const size_t bytes = (size_t)rows * width;
     if (width == desc_bytes) {
         SFM_CUDA(ctx, cudaMemcpyAsync((char*)mc.desc.p + (size_t)row0 * width, img, bytes, cudaMemcpyHostToDevice, ctx->stream));
@@ -596,32 +605,14 @@ int sfmb200_match_knn2_ratio(sfmb200_ctx* ctx, const uint8_t* q, int nq, const u
     MatchCache& mc = ctx->mcache;
     const char* env = getenv("SFMB200_MATCH_CACHE");
     const bool keep = !(env && env[0] == '0');
-    const int br = match_tc_block_rows();
-    if (mc.width != width || !keep) { mc.entries.clear(); mc.rows_used = 0; mc.blk_used = 0; mc.width = width; }
-    auto resident = [&](const uint8_t* p, int rows, uint64_t h) {
-        for (const MatchCacheEntry& e : mc.entries) if (e.host == p && e.rows == rows && e.desc_bytes == desc_bytes && e.hash == h) return true;
-        return false;
-    };
-    int64_t need_rows = 0; int need_blk = 0;
-    if (!resident(q, nq, hq)) { need_rows += nq; need_blk += ceil_div(nq, br); }
-    if (!resident(t, nt, ht) && !(t == q && nt == nq && ht == hq)) { need_rows += nt; need_blk += ceil_div(nt, br); }
-    if (width != 32) need_blk = 0;
-    if (mc.rows_used + need_rows > mc.rows_cap || mc.blk_used + need_blk > mc.blk_cap) {
-        // flush everything (simple and predictable), then grow if the pair alone does not fit
-        mc.entries.clear(); mc.rows_used = 0; mc.blk_used = 0;
-        need_rows = (int64_t)nq + nt; need_blk = width == 32 ? ceil_div(nq, br) + ceil_div(nt, br) : 0;
-        const int64_t want_rows = std::max<int64_t>(need_rows, 16 * 8192);          // room for >= 16 images of 8 k features
-        if (need_rows > mc.rows_cap || (size_t)mc.rows_cap * width > mc.desc.cap) {
-            SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            SFM_CUDA(ctx, mc.desc.reserve((size_t)want_rows * width + 16));
-            mc.rows_cap = want_rows;
-        }
-        const int want_blk = width == 32 ? std::max<int>(need_blk, (int)(want_rows / br) + 32) : 0;
-        if (want_blk > mc.blk_cap) {
-            SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            SFM_CUDA(ctx, mc.exp.reserve((size_t)want_blk * match_tc_block_bytes(false)));
-            mc.blk_cap = want_blk;
-        }
+    const MatchCachePlan plan = match_cache_plan(mc, mc.desc.cap, width, keep, desc_bytes, q, nq, hq, t, nt, ht, match_tc_block_rows(),
+                                                 match_tc_block_bytes(false));
+    if (plan.desc_bytes || plan.exp_bytes) {
+        SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        cudaError_t e = plan.desc_bytes ? mc.desc.reserve(plan.desc_bytes) : cudaSuccess;
+        if (e == cudaSuccess && plan.exp_bytes) e = mc.exp.reserve(plan.exp_bytes);
+        if (e != cudaSuccess) mc.reset();
+        SFM_CUDA(ctx, e);
     }
     PairDesc pd; pd.out_row = 0; pd.nq = nq; pd.nt = nt;
     int rc = cache_acquire(ctx, q, nq, desc_bytes, width, hq, pd.q_row, pd.q_blk);
@@ -632,7 +623,7 @@ int sfmb200_match_knn2_ratio(sfmb200_ctx* ctx, const uint8_t* q, int nq, const u
     int64_t ooff[2]; int32_t cnt[1];
     rc = match_pairs_host_out(ctx, (const uint32_t*)mc.desc.p, width == 32 ? (const uint8_t*)mc.exp.p : nullptr, width / 4, hp, nq, nq, nt, ratio,
                               out_q, out_t, out_d, ooff, cnt);
-    if (rc) { mc.entries.clear(); mc.rows_used = 0; mc.blk_used = 0; return rc; }
+    if (rc) { mc.flush(); return rc; }
     *out_n = cnt[0];
     return SFMB200_OK;
 }
