@@ -473,7 +473,7 @@ int sfmb200_orb_layout(int width, int height, int nfeatures, int32_t* level_w, i
 int sfmb200_orb_linear_exact_taps(int src, int dst, int32_t* i0, int32_t* i1, int32_t* weight);
 int sfmb200_orb_retain_best(const float* response, int n, int n_points, int32_t* order);
 /* Inspection of the last extraction (parity tests): one level of image `image` of the last batch; stage 0 = pyramid, 1 = blurred
- * pyramid the descriptors sample, 2 = FAST score map.  out [level_w * level_h]. */
+ * pyramid the descriptors sample, 2 = FAST score map.  out [level_w * level_h] with that image's own level size. */
 int sfmb200_orb_download_level(sfmb200_ctx* ctx, int stage, int image, int level, uint8_t* out);
 /* Host wall-clock (ms) of the phases of the last extraction call: 0 staging + upload + kernel enqueue, 1 wait for detection,
  * 2 candidate read-back, 3 first retainBest, 4 Harris round trip, 5 second retainBest, 6 describe round trip, 7 copy-out. */
@@ -535,6 +535,26 @@ int sfmb200_resize_batch(sfmb200_ctx* ctx, const uint8_t* const* src, const int*
                          double scale, uint8_t* const* dst, const size_t* dst_stride);
 int sfmb200_decode_jpeg_batch_scaled(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale,
                                      uint8_t* const* out_bgr, const size_t* out_stride);
+
+/* ---- f-3: JPEG files to ORB features in one call ----------------------------------------------------------------- */
+/*
+ * setImagesDirectory's imread (+ resize) loop and SfM::extractFeatures for all images of a run, with the images staying on the device
+ * between the decode and ORB: per image the key points and descriptors of
+ *     ORB::create(nfeatures)->detectAndCompute(resize(imread(file), Size(), scale, scale))      (no resize when scale == 1)
+ * bit-identical to OpenCV, exactly what sfmb200_decode_jpeg_batch[_scaled] followed by sfmb200_orb_detect_and_compute gives.  The
+ * images may differ in size (EXIF orientations 5-8 swap width and height); they share every launch.
+ *   data, size, n, scale   as in sfmb200_decode_jpeg_batch_scaled; the same statuses for unsupported or corrupt files, detected before
+ *                          any ORB work.  A decoded (resized) image with a side below 8 pixels returns SFMB200_ERR_INVALID, one over 2^28
+ *                          pixels SFMB200_ERR_UNSUPPORTED, before any launch; the message names the image.
+ *   keypoints, descriptors, n_keypoints   [n][max_keypoints] / [n][max_keypoints * 32] / [n], as in sfmb200_orb_detect_and_compute_batch
+ *                          (n_keypoints may exceed max_keypoints: call again with a larger capacity).
+ *   out_bgr, out_stride    NULL: the images are not downloaded.  Otherwise as in sfmb200_decode_jpeg_batch_scaled.
+ * n == 0 does nothing.  sfmb200_orb_last_timings and sfmb200_jpeg_last_stats describe this call; stats [6] counts only the bytes that
+ * were downloaded (the error words and statistics, plus the images if asked for).  sfmb200_orb_download_level inspects its last group.
+ */
+int sfmb200_decode_jpeg_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, int nfeatures,
+                                    int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
+                                    uint8_t* const* out_bgr /* NULL: images not downloaded */, const size_t* out_stride);
 
 /* ---- multi-GPU plumbing (NCCL, one process per GPU) ------------------------------------------------------ */
 #define SFMB200_UNIQUE_ID_BYTES 128

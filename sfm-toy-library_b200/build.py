@@ -68,7 +68,7 @@ def build_host(force=False):
     """C++ host shim (host/shim.cpp: the reference's three stage functions over the C ABI) + its test binary."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim.cpp", "sfmtoylib_b200.h", "sfm_features.h", "cv_min.h")] + [SO]
     if force or _stale(out, deps):
         r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", os.path.join(hdir, "shim.cpp"), os.path.join(hdir, "test_shim.cpp"),
                             "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib", "-lpthread", "-o", out],
@@ -83,7 +83,7 @@ def build_host_essential(force=False):
     """The shim built with SFMB200_SHIM_ESSENTIAL (findCameraMatricesFromMatch on the device too) + its test binary."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_essential")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_essential.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_essential.cpp", "sfmtoylib_b200.h", "sfm_features.h", "cv_min.h")] + [SO]
     if force or _stale(out, deps):
         r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", "-DSFMB200_SHIM_ESSENTIAL", os.path.join(hdir, "shim.cpp"),
                             os.path.join(hdir, "test_shim_essential.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
@@ -98,7 +98,7 @@ def build_host_homography(force=False):
     """The shim built with SFMB200_SHIM_HOMOGRAPHY (findHomographyInliers on the device too) + its test binary."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_homography")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_homography.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_homography.cpp", "sfmtoylib_b200.h", "sfm_features.h", "cv_min.h")] + [SO]
     if force or _stale(out, deps):
         r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", "-DSFMB200_SHIM_HOMOGRAPHY", os.path.join(hdir, "shim.cpp"),
                             os.path.join(hdir, "test_shim_homography.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
@@ -113,7 +113,7 @@ def build_host_pose(force=False):
     """The shim built with SFMB200_SHIM_POSE (findCameraPoseFrom2D3DMatch on the device too) + its test binary."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_pose")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_pose.cpp", "sfmtoylib_b200.h", "sfm_glue.h", "cv_min.h")] + [SO]
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_pose.cpp", "sfmtoylib_b200.h", "sfm_glue.h", "sfm_features.h", "cv_min.h")] + [SO]
     if force or _stale(out, deps):
         r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", "-DSFMB200_SHIM_POSE", os.path.join(hdir, "shim.cpp"),
                             os.path.join(hdir, "test_shim_pose.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
@@ -128,7 +128,7 @@ def build_images(force=False):
     """sfmtoylib::readImages (host/sfm_images.cpp: the imread loop of setImagesDirectory over sfmb200_decode_jpeg_batch) + its driver."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_images")
     os.makedirs(os.path.dirname(out), exist_ok=True)
-    deps = [os.path.join(hdir, f) for f in ("sfm_images.cpp", "sfm_images.h", "test_images.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
+    deps = [os.path.join(hdir, f) for f in ("sfm_images.cpp", "sfm_images.h", "sfm_features.h", "test_images.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
     if force or _stale(out, deps):
         r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", os.path.join(hdir, "sfm_images.cpp"), os.path.join(hdir, "test_images.cpp"),
                             "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib", "-lpthread", "-o", out],
@@ -136,6 +136,23 @@ def build_images(force=False):
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("readImages build failed")
+    return out
+
+
+def build_images_features(force=False):
+    """sfmtoylib::readImagesAndFeatures (host/sfm_images.cpp: decode, downscale and ORB in one sfmb200_decode_jpeg_extract_orb call) +
+    its driver."""
+    hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_images_features")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    deps = [os.path.join(hdir, f) for f in ("sfm_images.cpp", "sfm_images.h", "sfm_features.h", "test_images_features.cpp", "sfmtoylib_b200.h",
+                                            "cv_min.h")] + [SO]
+    if force or _stale(out, deps):
+        r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", os.path.join(hdir, "sfm_images.cpp"), os.path.join(hdir, "test_images_features.cpp"),
+                            "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib", "-lpthread", "-o", out],
+                           capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("readImagesAndFeatures build failed")
     return out
 
 
@@ -176,5 +193,6 @@ if __name__ == "__main__":
     print(build_host_homography(force="--force" in sys.argv))
     print(build_host_pose(force="--force" in sys.argv))
     print(build_images(force="--force" in sys.argv))
+    print(build_images_features(force="--force" in sys.argv))
     print(build_glue(force="--force" in sys.argv))
     print(build_ply(force="--force" in sys.argv))

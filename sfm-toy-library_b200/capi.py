@@ -490,6 +490,42 @@ class Context:
             self._check(lib().sfmb200_decode_jpeg_batch_scaled(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
         return outs
 
+    def decode_jpeg_orb(self, files, scale=1.0, nfeatures=5000, capacity=None, images=True):
+        """sfmb200_decode_jpeg_extract_orb: decode_jpeg(files, scale) and orb_detect_and_compute on every image in one call, with the
+        images staying on the device in between; they may differ in size.  Returns (images or None, [(key points, descriptors), ...]):
+        the images as decode_jpeg returns them when `images` is true (else they are not downloaded), and per image what
+        orb_detect_and_compute returns for it.  A capacity below a key point count repeats the call with the count."""
+        files = [bytes(f) for f in files]
+        n = len(files)
+        scale = float(scale)
+        if n == 0:
+            return ([] if images else None), []
+        outs = None
+        if images:
+            outs = []
+            for f in files:
+                rc, w, h, _ = jpeg_info(f)
+                if rc == 0 and scale != 1.0:
+                    w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
+                outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))
+        data = (C.c_char_p * n)(*files)
+        sizes = (C.c_size_t * n)(*[len(f) for f in files])
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs]) if images else None
+        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
+        while True:
+            kp = np.zeros((n, max(cap, 1), 7), np.float32); desc = np.zeros((n, max(cap, 1), 32), np.uint8); cnt = np.zeros(n, np.int32)
+            self._check(lib().sfmb200_decode_jpeg_extract_orb(self._h, data, sizes, n, C.c_double(scale), int(nfeatures), cap,
+                                                              _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32), ptrs, None))
+            if cnt.max(initial=0) <= cap:
+                break
+            cap = int(cnt.max())                      # ties at a selection threshold: more key points than asked for
+        feats = []
+        for i in range(n):
+            k = kp[i, :cnt[i]].copy()
+            k[:, 5:7] = k[:, 5:7].view(np.int32).astype(np.float32)      # octave, class_id are int32 in the record
+            feats.append((k, desc[i, :cnt[i]].copy()))
+        return outs, feats
+
     def resize_images(self, images, scale):
         """sfmb200_resize_batch: `images` is a list of uint8 [h, w, 3] B,G,R arrays (any sizes, strided rows allowed); returns them
         resized by `scale`, byte-identical to cv2.resize(img, None, fx=scale, fy=scale) (INTER_LINEAR), in one call.  A refused scale

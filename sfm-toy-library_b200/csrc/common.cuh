@@ -74,8 +74,12 @@ struct MatchCache : MatchCacheState {
     void release() { desc.release(); exp.release(); reset(); }
 };
 
-// Device buffers of the last ORB extraction (orb.cu), kept for sfmb200_orb_download_level (stage-by-stage parity tests).
-struct OrbLast { uint8_t *pyr = nullptr, *blur = nullptr, *score = nullptr; int slab = 0, nimg = 0, w = 0, h = 0, nfeatures = 0; };
+// Device buffers of the last ORB extraction group (orb.cu), kept for sfmb200_orb_download_level (stage-by-stage parity tests): the
+// size of each of its images and where that image's pyramid starts in the three arenas.
+struct OrbLast {
+    uint8_t *pyr = nullptr, *blur = nullptr, *score = nullptr; int nimg = 0, nfeatures = 0;
+    std::vector<int> w, h; std::vector<size_t> pix0;
+};
 
 // Device memory of one descriptor set (match.cu), kept by the context between sets: SfM::createFeatureMatchMatrix builds one set per run and
 // a benchmark one per repetition -- cudaMalloc / cudaFree (a device-wide synchronisation each) cost more than matching 21 image pairs.
@@ -102,6 +106,7 @@ struct sfmb200_ctx {
     DescWorkspace ds_ws;        // cached device memory of a descriptor set
     DevBuf orb_dev, orb_lists;  // ORB extraction: pyramids / score maps / candidates of a batch of images; key point lists
     PinBuf orb_pin_img, orb_pin_a, orb_pin_b, orb_pin_c;   // ORB extraction: pinned image staging / staging of the three host round trips
+    PinBuf orb_pin_tab;         // ORB extraction: a group's layouts, resize taps and tile lists, staged for their one upload
     double orb_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};            // host wall-clock of the phases of the last extraction (sfmb200_orb_last_timings)
     HostPool* pool = nullptr;   // host threads for the work that stays on the CPU (created on first use)
     OrbLast orb_last;
@@ -169,6 +174,11 @@ void sfmb200_comm_destroy(sfmb200_ctx* ctx);
 // image downscale (resize.cu), also run by the scaled JPEG decode (jpeg.cu) on the images it has just decoded.
 // rz_plan: fills dw, dh, the tap offsets and the tiles of imgs[0..n) (sw, sh set by the caller) and appends their taps; false and the
 // image in *bad if a size is refused.  rz_enqueue: one launch on ctx->stream over device copies of imgs / taps.
+// ORB extraction of images already on the device (orb.cu): packed B,G,R rows of ws[i] x hs[i] pixels at d_bgr[i], any sizes; results as
+// sfmb200_orb_detect_and_compute_batch.  The caller holds ctx->mu and has checked the sizes.
+int orb_extract_device(sfmb200_ctx* ctx, const uint8_t* const* d_bgr, const int* ws, const int* hs, int n, int nfeatures, int max_keypoints,
+                       sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints);
+
 struct RzImg; struct RzTap;
 bool rz_plan(double scale, RzImg* imgs, int n, std::vector<RzTap>& taps, int* bad);
 int rz_enqueue(sfmb200_ctx* ctx, double scale, const RzImg* imgs, int n, const RzImg* d_imgs, const RzTap* d_taps, const uint8_t* d_src,

@@ -83,7 +83,7 @@ void sfmb200_destroy(sfmb200_ctx* ctx) {
     ctx->ipc_cache.clear();
     sfmb200_comm_destroy(ctx);
     ctx->orb_dev.release(); ctx->orb_lists.release();
-    ctx->orb_pin_img.release(); ctx->orb_pin_a.release(); ctx->orb_pin_b.release(); ctx->orb_pin_c.release();
+    ctx->orb_pin_img.release(); ctx->orb_pin_a.release(); ctx->orb_pin_b.release(); ctx->orb_pin_c.release(); ctx->orb_pin_tab.release();
     delete ctx->pool; ctx->pool = nullptr;
     if (ctx->orb_stream) cudaStreamDestroy(ctx->orb_stream);
     if (ctx->orb_up) cudaStreamDestroy(ctx->orb_up);

@@ -348,12 +348,18 @@ size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 }  // namespace
 
-// Both decode entry points.  scale == 1: jd_color writes the images into the download area.  Otherwise jd_color writes them to device
-// memory, resize.cu's kernels downscale them into the download area, and only the resized images come back.
+// Images a decode leaves on the device (jd_decode with `res`): packed B,G,R rows of w[i] x h[i] pixels at ptr[i], inside ctx->jpeg_dev,
+// valid until the next decode.
+struct JdResident { std::vector<const uint8_t*> ptr; std::vector<int> w, h; };
+
+// Every decode entry point.  scale == 1: jd_color writes the images into the download area.  Otherwise jd_color writes them to device
+// memory, resize.cu's kernels downscale them into the download area, and only the resized images come back.  With `res` the images
+// also stay where they are for the caller, each refused unless ORB can take it (8 <= width, height; at most 2^28 pixels), and out_bgr
+// may be null: then only the error words and the statistics come back.
 static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
-                     const size_t* out_stride) {
+                     const size_t* out_stride, JdResident* res = nullptr) {
     if (!ctx) return SFMB200_ERR_INVALID;
-    if (n < 0 || (n > 0 && (!data || !size || !out_bgr))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: bad arguments");
+    if (n < 0 || (n > 0 && (!data || !size || (!out_bgr && !res)))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: bad arguments");
     if (n > 65535) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: at most 65535 images per call");
     if (!std::isfinite(scale) || scale <= 0)
         return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch_scaled: scale %g is not a positive finite number", scale);
@@ -371,7 +377,7 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     pool.parallel_for(n, [&](int i) { rcs[i] = jp_parse(data[i], size[i], JD_CHUNK, ims[i], whys[i]); });
     for (int i = 0; i < n; ++i) {
         if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", i, whys[i].c_str());
-        if (!out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", i);
+        if (out_bgr && !out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", i);
     }
     // ---- the downscale: output sizes and taps of every image
     std::vector<RzImg> rz(scaled ? n : 0);
@@ -383,9 +389,13 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
             return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", bad, scale, ims[bad].OW, ims[bad].OH);
     }
     for (int i = 0; i < n; ++i) {
-        const int ow = scaled ? rz[i].dw : ims[i].OW;
-        if (out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
+        const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
+        if (out_bgr && out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
             return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", i, out_stride[i], ow * 3);
+        if (res && (ow < 8 || oh < 8))
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: a %dx%d image is below ORB's minimum of 8 pixels per side", i, ow, oh);
+        if (res && (int64_t)ow * oh > ((int64_t)1 << 28))
+            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image %d: a %dx%d image is too large for ORB (limit 2^28 pixels)", i, ow, oh);
     }
 
     // ---- layout
@@ -542,21 +552,30 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     SFM_LAUNCH_CHECK(ctx);
     if (scaled)
         if (int rc = rz_enqueue(ctx, scale, rz.data(), n, (const RzImg*)(dv + o_rzimg), (const RzTap*)(dv + o_rztap), d_full, d_out)) return rc;
-    SFM_CUDA(ctx, ctx->jpeg_pin_down.reserve(down_bytes));
+    const size_t got = out_bgr ? down_bytes : o_out;                 // images left on the device only: the error words and statistics
+    SFM_CUDA(ctx, ctx->jpeg_pin_down.reserve(got));
     char* hd = (char*)ctx->jpeg_pin_down.p;
-    SFM_CUDA(ctx, cudaMemcpyAsync(hd, down, down_bytes, cudaMemcpyDeviceToHost, st));
+    SFM_CUDA(ctx, cudaMemcpyAsync(hd, down, got, cudaMemcpyDeviceToHost, st));
     SFM_CUDA(ctx, cudaStreamSynchronize(st));
 
     const JdStats* hs = (const JdStats*)(hd + o_stats);
     ctx->jpeg_stats[0] = nsub; ctx->jpeg_stats[1] = hs->cw_first; ctx->jpeg_stats[2] = hs->cw_extra;
     ctx->jpeg_stats[3] = hs->rounds; ctx->jpeg_stats[4] = hs->swept;
-    ctx->jpeg_stats[5] = (int64_t)up_bytes; ctx->jpeg_stats[6] = (int64_t)down_bytes;
+    ctx->jpeg_stats[5] = (int64_t)up_bytes; ctx->jpeg_stats[6] = (int64_t)got;
     const int* herr = (const int*)(hd + o_err);
     for (int i = 0; i < n; ++i)
         if (herr[i])
             return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: %s", i,
                                 herr[i] & JD_ERR_DATA ? "corrupt entropy-coded data (no Huffman code, overrun or a run past coefficient 63)"
                                                       : "entropy-coded data ends before the last block");
+    if (res) {
+        res->ptr.resize(n); res->w.resize(n); res->h.resize(n);
+        for (int i = 0; i < n; ++i) {
+            res->ptr[i] = d_out + (scaled ? rz[i].dst0 : img[i].out0);
+            res->w[i] = scaled ? rz[i].dw : img[i].OW; res->h[i] = scaled ? rz[i].dh : img[i].OH;
+        }
+    }
+    if (!out_bgr) return SFMB200_OK;
     pool.parallel_for(n, [&](int i) {
         const int ow = scaled ? rz[i].dw : img[i].OW, oh = scaled ? rz[i].dh : img[i].OH;
         const size_t row = (size_t)ow * 3, stride = out_stride && out_stride[i] ? out_stride[i] : row;
@@ -593,6 +612,21 @@ int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, cons
 int sfmb200_decode_jpeg_batch_scaled(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale,
                                      uint8_t* const* out_bgr, const size_t* out_stride) {
     return jd_decode(ctx, data, size, n, scale, out_bgr, out_stride);
+}
+
+int sfmb200_decode_jpeg_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, int nfeatures,
+                                    int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
+                                    uint8_t* const* out_bgr, const size_t* out_stride) {
+    if (!ctx) return SFMB200_ERR_INVALID;
+    if (n < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_extract_orb: n < 0");
+    if (n == 0) return SFMB200_OK;
+    if (!keypoints || !descriptors || !n_keypoints || max_keypoints < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_extract_orb: null buffer");
+    if (nfeatures < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "nfeatures < 0");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    // The decode reads back its error words (with the images, if asked for) and fails on a bad file before ORB launches anything.
+    JdResident res;
+    if (int rc = jd_decode(ctx, data, size, n, scale, out_bgr, out_stride, &res)) return rc;
+    return orb_extract_device(ctx, res.ptr.data(), res.w.data(), res.h.data(), n, nfeatures, max_keypoints, keypoints, descriptors, n_keypoints);
 }
 
 }  // extern "C"

@@ -11,61 +11,27 @@
 // `KeyPointsFilter::retainBest` selections stay on the host ON PURPOSE: their result ORDER is whatever libstdc++'s std::nth_element +
 // std::partition leave behind, and every later stage (and the matcher's trainIdx) inherits that order -- running the same two
 // algorithms on 8-byte (response, index) records reproduces it exactly and costs ~0.1 ms per image.
-// All kernels carry the image index in blockIdx.z / the record, so a batch of equally sized images shares every launch and
-// every host<->device round trip (3 per batch).
+// All kernels carry the image index in blockIdx.z, the tile list or the record and look up that image's layout (sizes and arena
+// offsets, orb_groups.h) in a device table, so a group of images of any sizes shares every launch and every host<->device round trip
+// (3 per group).  The images come from host memory (staged and uploaded here) or are already on the device (sfmb200_decode_jpeg_extract_orb).
 //
 // Integer / byte work, HBM- and latency-bound (2.6 MB of pyramid per 1024x768 image): no tensor cores involved.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <map>
 #include <memory>
 
 #include "common.cuh"
+#include "orb_groups.h"
 #include "orb_math.cuh"
 #define ORB_PATTERN_DECL __device__
 #include "orb_pattern.h"
 
 namespace {
 
-constexpr int ORB_LEVELS = 8;
 constexpr int ORB_EDGE = 31;          // edgeThreshold
 constexpr int ORB_FAST_T = 20;        // fastThreshold
-constexpr int CHUNK = 32;             // pixels per survivor-mask word
-
-struct OrbLevel { int w, h, off, row0; float scale, inv_scale; int quota, pad; };
-struct OrbLayout {
-    OrbLevel lv[ORB_LEVELS];
-    int total_rows;      // rows of all levels
-    int slab;            // bytes of one image's pyramid (levels back to back, each 16-byte aligned)
-    int chunks;          // survivor-mask words per row = ceil(level-0 width / 32), the same stride for every level
-    int ncnt;            // total_rows * chunks
-};
-
-// ---------------------------------------------------------------------------------------------------- host-side layout (pure functions)
-// ORB_Impl::detectAndCompute: layerScale[l] = (float)pow((double)1.2f, l); layer size = cvRound(cols / scale) x cvRound(rows / scale);
-// computeKeyPoints: nfeaturesPerLevel from the geometric series with factor 1 / 1.2f.
-int make_layout(int w, int h, int nfeatures, OrbLayout& L) {
-    const double sf = (double)1.2f;
-    int off = 0, row = 0;
-    const float factor = (float)(1.0 / sf);
-    float ndesired = (float)nfeatures * (1.0f - factor) / (1.0f - (float)std::pow((double)factor, (double)ORB_LEVELS));
-    int sum = 0;
-    for (int l = 0; l < ORB_LEVELS; l++) {
-        OrbLevel& v = L.lv[l];
-        v.scale = (float)std::pow(sf, (double)l);
-        v.inv_scale = 1.0f / v.scale;
-        v.w = (int)std::nearbyintf((float)w / v.scale); v.h = (int)std::nearbyintf((float)h / v.scale);
-        if (v.w < 0) v.w = 0;
-        if (v.h < 0) v.h = 0;
-        if (v.w == 0 || v.h == 0) v.w = v.h = 0;
-        v.off = off; v.row0 = row; v.pad = 0;
-        off += (v.w * v.h + 15) & ~15; row += v.h;
-        if (l < ORB_LEVELS - 1) { v.quota = (int)std::nearbyintf(ndesired); sum += v.quota; ndesired *= factor; }
-        else v.quota = std::max(nfeatures - sum, 0);
-    }
-    L.total_rows = row; L.slab = (off + 255) & ~255; L.chunks = ceil_div(w, CHUNK); L.ncnt = L.total_rows * L.chunks;
-    return 0;
-}
 
 // resize(INTER_LINEAR_EXACT) tap tables: for destination index d, the two source indices and the weight (1/256) of the second one.
 void linear_exact_taps(int src, int dst, int32_t* i0, int32_t* i1, int32_t* a) {
@@ -96,24 +62,34 @@ void retain_best(std::vector<Rec>& k, int n_points) {
 }
 
 // ---------------------------------------------------------------------------------------------------- kernels
-__global__ void __launch_bounds__(256) orb_gray_kernel(const uint8_t* __restrict__ raw, size_t raw_stride_img, int row_stride, int w, int h,
-                                                        uint8_t* __restrict__ pyr, int slab) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, img = blockIdx.z;
-    if (x >= w) return;
-    const uint8_t* p = raw + (size_t)img * raw_stride_img + (size_t)y * row_stride + 3 * x;
-    pyr[(size_t)img * slab + (size_t)y * w + x] = (uint8_t)orbm::gray_from_bgr(p[0], p[1], p[2]);
+// Tile lists of the FAST and blur kernels: one 32-bit word per tile row of a group, image slot << 16 | level << 13 | first row / 16.
+// The grid is flat: block b works on tile b / xblocks and 32- or 64-pixel column b % xblocks, with xblocks from the group's widest image.
+__host__ __device__ __forceinline__ uint32_t tile_word(int slot, int l, int y0) { return (uint32_t)slot << 16 | (uint32_t)l << 13 | (uint32_t)(y0 >> 4); }
+
+// grid = (columns of the widest image / 256, rows of the tallest, images); Ls = the layouts of the launch's images
+__global__ void __launch_bounds__(256) orb_gray_kernel(const OrbLayout* __restrict__ Ls, uint8_t* __restrict__ pyr) {
+    const OrbLayout& L = Ls[blockIdx.z];
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, w = L.lv[0].w;
+    if (x >= w || y >= L.lv[0].h) return;
+    const uint8_t* p = L.src + (size_t)y * L.src_stride + 3 * x;
+    pyr[L.pix0 + (size_t)y * w + x] = (uint8_t)orbm::gray_from_bgr(p[0], p[1], p[2]);
 }
 
-__global__ void __launch_bounds__(256) orb_resize_kernel(uint8_t* pyr, int slab, int src_off, int sw, int dst_off, int dw, int dh,
-                                                          const int32_t* __restrict__ taps /* x: i0,i1,a [dw each]; y: i0,i1,a [dh each] */) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, img = blockIdx.z;
-    if (x >= dw) return;
+// level l from level l - 1; taps (x: i0,i1,a [dw each]; y: i0,i1,a [dh each]) at the level's offset in the group's table
+__global__ void __launch_bounds__(256) orb_resize_kernel(const OrbLayout* __restrict__ Ls, uint8_t* pyr, int l, const int32_t* __restrict__ taps_all) {
+    const OrbLayout& L = Ls[blockIdx.z];
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    const OrbLevel& d = L.lv[l];
+    const int dw = d.w, dh = d.h;
+    if (x >= dw || y >= dh) return;
+    const int sw = L.lv[l - 1].w;
+    const int32_t* taps = taps_all + d.taps;
     const int x0 = taps[x], x1 = taps[dw + x], ax = taps[2 * dw + x];
     const int32_t* ty = taps + 3 * dw;
     const int y0 = ty[y], y1 = ty[dh + y], ay = ty[2 * dh + y];
-    const uint8_t* s = pyr + (size_t)img * slab + src_off;
+    const uint8_t* s = pyr + L.pix0 + L.lv[l - 1].off;
     const int v = orbm::resize_linear_exact(s[(size_t)y0 * sw + x0], s[(size_t)y0 * sw + x1], s[(size_t)y1 * sw + x0], s[(size_t)y1 * sw + x1], ax, ay);
-    pyr[(size_t)img * slab + dst_off + (size_t)y * dw + x] = (uint8_t)v;
+    pyr[L.pix0 + d.off + (size_t)y * dw + x] = (uint8_t)v;
 }
 
 // FAST-9/16: the four compass points decide whether a position can be a corner at all (9-18 % of the pixels of a photograph pass, but
@@ -139,22 +115,27 @@ __device__ __forceinline__ int fast_full(const uint8_t* __restrict__ I, int w, i
 // survivors per pyramid row (integer atomics: order-independent).  The tile is 32 rows high so that the dense candidate list (~150 of
 // 1156 positions) fills the CTA's 8 warps in the scoring phase -- with 8-row tiles two warps scored while six waited at the barrier
 // (ncu: barrier = top stall) -- and the halo costs 13 % instead of 33 %.
-// grid = (words per row of level 0, tile rows of all levels, images), block = (32, 8): thread (x, y) owns rows y, y+8, y+16, y+24.
+// grid = xblocks (survivor words per row of the widest image) x tile rows of the launch's images, block = (32, 8): thread (x, y) owns
+// rows y, y+8, y+16, y+24.
 constexpr int FT_W = 32, FT_H = 32, FT_TY = 8, FT_N = (FT_W + 2) * (FT_H + 2);
 __global__ void __launch_bounds__(FT_W * FT_TY) orb_fast_nms_kernel(const uint8_t* __restrict__ pyr, uint8_t* __restrict__ score, uint32_t* __restrict__ mask,
-                                                                     int32_t* __restrict__ row_cnt, OrbLayout L, const int32_t* __restrict__ tile_lvl,
-                                                                     const int32_t* __restrict__ tile_y0) {
+                                                                     int32_t* __restrict__ row_cnt, const OrbLayout* __restrict__ Ls,
+                                                                     const uint32_t* __restrict__ tiles, int xblocks) {
     __shared__ uint8_t sc[FT_H + 2][FT_W + 2 + 2];
     __shared__ uint16_t list[FT_N];
     __shared__ int nlist;
-    const int l = tile_lvl[blockIdx.y], y0 = tile_y0[blockIdx.y], x0 = blockIdx.x * FT_W, img = blockIdx.z;
-    const int w = L.lv[l].w, h = L.lv[l].h;
+    const uint32_t tile = tiles[blockIdx.x / xblocks];
+    const int bx = blockIdx.x % xblocks, l = (tile >> 13) & 7, y0 = (int)(tile & 0x1FFF) << 4, x0 = bx * FT_W;
+    const OrbLayout& L = Ls[tile >> 16];
+    if (bx >= L.chunks) return;                      // past this image's own words
+    const int w = L.lv[l].w, h = L.lv[l].h, row0 = L.lv[l].row0, chunks = L.chunks;
+    uint32_t* M = mask + L.mask0;
     if (x0 >= w) {                                   // words beyond this level's width: the scatter walks all `chunks` words of a row
         if (threadIdx.x == 0)
-            for (int ry = threadIdx.y; ry < FT_H && y0 + ry < h; ry += FT_TY) mask[(size_t)img * L.ncnt + (size_t)(L.lv[l].row0 + y0 + ry) * L.chunks + blockIdx.x] = 0u;
+            for (int ry = threadIdx.y; ry < FT_H && y0 + ry < h; ry += FT_TY) M[(size_t)(row0 + y0 + ry) * chunks + bx] = 0u;
         return;
     }
-    const uint8_t* I = pyr + (size_t)img * L.slab + L.lv[l].off;
+    const uint8_t* I = pyr + L.pix0 + L.lv[l].off;
     const int tid = threadIdx.y * FT_W + threadIdx.x;
     if (tid == 0) nlist = 0;
     __syncthreads();
@@ -170,13 +151,14 @@ __global__ void __launch_bounds__(FT_W * FT_TY) orb_fast_nms_kernel(const uint8_
     }
     __syncthreads();
     const int x = x0 + threadIdx.x;
+    uint8_t* S = score + L.pix0 + L.lv[l].off;
 #pragma unroll
     for (int ry = threadIdx.y; ry < FT_H; ry += FT_TY) {
         const int y = y0 + ry;
         const int s = sc[ry + 1][threadIdx.x + 1];
         bool keep = false;
         if (x < w && y < h) {
-            score[(size_t)img * L.slab + L.lv[l].off + (size_t)y * w + x] = (uint8_t)s;
+            S[(size_t)y * w + x] = (uint8_t)s;
             if (s && x >= ORB_EDGE && x < w - ORB_EDGE && y >= ORB_EDGE && y < h - ORB_EDGE) {
                 const uint8_t* r0 = &sc[ry][threadIdx.x]; const uint8_t* r1 = r0 + (FT_W + 4); const uint8_t* r2 = r1 + (FT_W + 4);
                 keep = s > r0[0] && s > r0[1] && s > r0[2] && s > r1[0] && s > r1[2] && s > r2[0] && s > r2[1] && s > r2[2];
@@ -184,24 +166,27 @@ __global__ void __launch_bounds__(FT_W * FT_TY) orb_fast_nms_kernel(const uint8_
         }
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (threadIdx.x == 0 && y < h) {
-            const int row = L.lv[l].row0 + y;
-            mask[(size_t)img * L.ncnt + (size_t)row * L.chunks + blockIdx.x] = m;
-            if (m) atomicAdd(&row_cnt[(size_t)img * (L.total_rows + 1) + row], __popc(m));
+            const int row = row0 + y;
+            M[(size_t)row * chunks + bx] = m;
+            if (m) atomicAdd(&row_cnt[L.cnt0 + row], __popc(m));
         }
     }
 }
 
 // Exclusive scan of the survivors per pyramid row of one image (one CTA per image); start of every level and the total.
-__global__ void __launch_bounds__(1024) orb_scan_kernel(const int32_t* __restrict__ row_cnt, int32_t* __restrict__ row_off, int32_t* __restrict__ lvl_start, OrbLayout L) {
+__global__ void __launch_bounds__(1024) orb_scan_kernel(const int32_t* __restrict__ row_cnt, int32_t* __restrict__ row_off, int32_t* __restrict__ lvl_start,
+                                                        const OrbLayout* __restrict__ Ls) {
     __shared__ int warp_sum[32];
     __shared__ int carry;
     const int img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int32_t* c = row_cnt + (size_t)img * (L.total_rows + 1); int32_t* o = row_off + (size_t)img * (L.total_rows + 1);
+    const OrbLayout& L = Ls[img];
+    const int total_rows = L.total_rows;
+    const int32_t* c = row_cnt + L.cnt0; int32_t* o = row_off + L.cnt0;
     if (tid == 0) carry = 0;
     __syncthreads();
-    for (int base = 0; base < L.total_rows; base += 1024) {
+    for (int base = 0; base < total_rows; base += 1024) {
         const int r = base + tid;
-        const int v = r < L.total_rows ? c[r] : 0;
+        const int v = r < total_rows ? c[r] : 0;
         int s = v;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(0xffffffffu, s, d); if (lane >= d) s += t; }
@@ -215,32 +200,34 @@ __global__ void __launch_bounds__(1024) orb_scan_kernel(const int32_t* __restric
         }
         __syncthreads();
         const int before = carry + (wid ? warp_sum[wid - 1] : 0) + s - v;
-        if (r < L.total_rows) o[r] = before;
+        if (r < total_rows) o[r] = before;
         __syncthreads();
         if (tid == 1023) carry = before + v;
         __syncthreads();
     }
-    if (tid == 0) o[L.total_rows] = carry;
+    if (tid == 0) o[total_rows] = carry;
     __syncthreads();
     if (tid <= ORB_LEVELS) lvl_start[img * 16 + tid] = (tid < ORB_LEVELS && L.lv[tid].h > 0) ? o[L.lv[tid].row0] : carry;
 }
 
 // Ordered scatter: one warp per pyramid row -> candidates (x | y << 16, score | level << 16), raster order inside a level (the order cv::FAST
-// emits), levels back to back.
+// emits), levels back to back.  grid = (rows of the image with the most pyramid rows / 8, 1, images)
 __global__ void __launch_bounds__(256) orb_scatter_kernel(const uint32_t* __restrict__ mask, const uint8_t* __restrict__ score, const int32_t* __restrict__ row_off,
-                                                           OrbLayout L, uint2* __restrict__ cand, int cand_cap) {
-    const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, img = blockIdx.z;
+                                                           const OrbLayout* __restrict__ Ls, uint2* __restrict__ cand) {
+    const OrbLayout& L = Ls[blockIdx.z];
+    const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (row >= L.total_rows) return;
     int l = 0;
 #pragma unroll
     for (int i = 1; i < ORB_LEVELS; i++) l += (L.lv[i].h > 0 && row >= L.lv[i].row0) ? 1 : 0;
-    const int w = L.lv[l].w, y = row - L.lv[l].row0;
-    const uint8_t* sc = score + (size_t)img * L.slab + L.lv[l].off + (size_t)y * w;
-    int pos = row_off[(size_t)img * (L.total_rows + 1) + row];
-    uint2* out = cand + (size_t)img * cand_cap;
-    for (int j0 = 0; j0 < L.chunks; j0 += 32) {
+    const int w = L.lv[l].w, y = row - L.lv[l].row0, chunks = L.chunks, cand_cap = L.cand_cap;
+    const uint8_t* sc = score + L.pix0 + L.lv[l].off + (size_t)y * w;
+    int pos = row_off[L.cnt0 + row];
+    uint2* out = cand + L.cand0;
+    const uint32_t* M = mask + L.mask0 + (size_t)row * chunks;
+    for (int j0 = 0; j0 < chunks; j0 += 32) {
         const int j = j0 + lane;
-        unsigned m = j < L.chunks ? mask[(size_t)img * L.ncnt + (size_t)row * L.chunks + j] : 0u;
+        unsigned m = j < chunks ? M[j] : 0u;
         const int c = __popc(m);
         int incl = c;
 #pragma unroll
@@ -257,14 +244,15 @@ __global__ void __launch_bounds__(256) orb_scatter_kernel(const uint32_t* __rest
 }
 
 // Harris response of selected candidates: one warp per record {x | y << 16, level | img << 8}.
-__global__ void __launch_bounds__(256) orb_harris_kernel(const uint8_t* __restrict__ pyr, OrbLayout L, const uint2* __restrict__ sel, int n,
+__global__ void __launch_bounds__(256) orb_harris_kernel(const uint8_t* __restrict__ pyr, const OrbLayout* __restrict__ Ls, const uint2* __restrict__ sel, int n,
                                                           float* __restrict__ response) {
     const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (i >= n) return;
     const uint2 r = sel[i];
     const int x = r.x & 0xFFFF, y = r.x >> 16, l = r.y & 0xFF, img = r.y >> 8;
+    const OrbLayout& L = Ls[img];
     const int w = L.lv[l].w;
-    const uint8_t* I = pyr + (size_t)img * L.slab + L.lv[l].off;
+    const uint8_t* I = pyr + L.pix0 + L.lv[l].off;
     int a = 0, b = 0, c = 0;
     for (int k = lane; k < 49; k += 32) {
         const uint8_t* p = I + (size_t)(y - 3 + k / 7) * w + (x - 3 + k % 7);
@@ -277,18 +265,20 @@ __global__ void __launch_bounds__(256) orb_harris_kernel(const uint8_t* __restri
     if (lane == 0) response[i] = orbm::harris_response(a, b, c);
 }
 
-// Float separable Gaussian of every level (BORDER_REFLECT_101).  Tile 64 x 16 per CTA; grid = (ceil(w0/64), ceil(h_l/16) summed over levels, images)
+// Float separable Gaussian of every level (BORDER_REFLECT_101).  Tile 64 x 16 per CTA; grid = xblocks (64-pixel columns of the widest
+// image) x tile rows (16 rows each) of the launch's images.
 constexpr int BT_W = 64, BT_H = 16;
 __device__ __forceinline__ int reflect101(int i, int n) { i = i < 0 ? -i : i; return i >= n ? 2 * n - 2 - i : i; }
-__global__ void __launch_bounds__(256) orb_blur_kernel(const uint8_t* __restrict__ pyr, uint8_t* __restrict__ blur, OrbLayout L,
-                                                        const int32_t* __restrict__ tile_lvl /* [grid.y] level of the tile row */,
-                                                        const int32_t* __restrict__ tile_y0 /* [grid.y] first row of the tile */) {
+__global__ void __launch_bounds__(256) orb_blur_kernel(const uint8_t* __restrict__ pyr, uint8_t* __restrict__ blur, const OrbLayout* __restrict__ Ls,
+                                                        const uint32_t* __restrict__ tiles, int xblocks) {
     __shared__ float R[BT_H + 6][BT_W];
-    const int l = tile_lvl[blockIdx.y], y0 = tile_y0[blockIdx.y], x0 = blockIdx.x * BT_W, img = blockIdx.z;
+    const uint32_t tile = tiles[blockIdx.x / xblocks];
+    const int l = (tile >> 13) & 7, y0 = (int)(tile & 0x1FFF) << 4, x0 = (blockIdx.x % xblocks) * BT_W;
+    const OrbLayout& L = Ls[tile >> 16];
     const int w = L.lv[l].w, h = L.lv[l].h;
     if (x0 >= w) return;
-    const uint8_t* I = pyr + (size_t)img * L.slab + L.lv[l].off;
-    uint8_t* O = blur + (size_t)img * L.slab + L.lv[l].off;
+    const uint8_t* I = pyr + L.pix0 + L.lv[l].off;
+    uint8_t* O = blur + L.pix0 + L.lv[l].off;
     if (w < 4 || h < 4) {                               // too small to reflect: copy (such a level cannot hold a key point anyway)
         for (int t = threadIdx.x; t < BT_W * BT_H; t += 256) {
             const int x = x0 + t % BT_W, y = y0 + t / BT_W;
@@ -324,7 +314,7 @@ __global__ void __launch_bounds__(256) orb_blur_kernel(const uint8_t* __restrict
 struct KeyPointOut { float x, y, size, angle, response; int32_t octave, class_id; };
 
 // ICAngles + computeOrbDescriptors + the final `pt *= scale`: one warp per key point record {x | y << 16, level | img << 8}.
-__global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur, OrbLayout L,
+__global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur, const OrbLayout* __restrict__ Ls,
                                                             const uint2* __restrict__ sel, const float* __restrict__ response, int n,
                                                             KeyPointOut* __restrict__ kp, uint8_t* __restrict__ desc) {
     __shared__ signed char pat[1024];
@@ -334,8 +324,9 @@ __global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __rest
     if (i >= n) return;
     const uint2 r = sel[i];
     const int x = r.x & 0xFFFF, y = r.x >> 16, l = r.y & 0xFF, img = r.y >> 8;
+    const OrbLayout& L = Ls[img];
     const int w = L.lv[l].w;
-    const uint8_t* I = pyr + (size_t)img * L.slab + L.lv[l].off;
+    const uint8_t* I = pyr + L.pix0 + L.lv[l].off;
     // intensity centroid over the circular patch of radius 15: lane = row v + 15
     int m10 = 0, m01 = 0;
     if (lane < 31) {
@@ -358,7 +349,7 @@ __global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __rest
     const int cx = orbm::round_even(orbm::mul(px, inv)), cy = orbm::round_even(orbm::mul(py, inv));
     float a, b;
     orbm::angle_to_cs(angle, &a, &b);
-    const uint8_t* C = blur + (size_t)img * L.slab + L.lv[l].off + (size_t)cy * w + cx;
+    const uint8_t* C = blur + L.pix0 + L.lv[l].off + (size_t)cy * w + cx;
     unsigned byte = 0;
 #pragma unroll
     for (int bit = 0; bit < 8; bit++) {
@@ -370,22 +361,21 @@ __global__ void __launch_bounds__(256) orb_describe_kernel(const uint8_t* __rest
     desc[(size_t)i * 32 + lane] = (uint8_t)byte;
 }
 
-
 // ---------------------------------------------------------------------------------------------------- host driver
+// One image size: its layout (arena offsets zero), its resize taps (per level l >= 1: x taps (3 * w_l) then y taps (3 * h_l); lv[l].taps
+// counts from the start of this vector) and the tile rows of the blur (BT_H rows) and FAST (FT_H rows) kernels as tile words of slot 0.
 struct OrbPlan {
     OrbLayout L;
-    std::vector<int32_t> taps;        // per level l >= 1: x taps (3 * w_l) then y taps (3 * h_l)
-    int taps_off[ORB_LEVELS];
-    std::vector<int32_t> blur_lvl, blur_y0;   // blur kernel: level and first row of every tile row (BT_H rows)
-    std::vector<int32_t> fast_lvl, fast_y0;   // FAST kernel: the same for FT_H rows
+    std::vector<int32_t> taps;
+    std::vector<uint32_t> blur_tiles, fast_tiles;
 };
 
 void make_plan(int w, int h, int nfeatures, OrbPlan& P) {
     make_layout(w, h, nfeatures, P.L);
     P.taps.clear();
     for (int l = 0; l < ORB_LEVELS; l++) {
-        P.taps_off[l] = (int)P.taps.size();
-        const OrbLevel& d = P.L.lv[l];
+        OrbLevel& d = P.L.lv[l];
+        d.taps = (int)P.taps.size();
         if (l == 0 || d.w == 0) continue;
         const OrbLevel& s = P.L.lv[l - 1];
         const size_t at = P.taps.size();
@@ -395,21 +385,312 @@ void make_plan(int w, int h, int nfeatures, OrbPlan& P) {
         t += 3 * d.w;
         linear_exact_taps(s.h, d.h, t, t + d.h, t + 2 * d.h);
     }
-    P.blur_lvl.clear(); P.blur_y0.clear(); P.fast_lvl.clear(); P.fast_y0.clear();
+    P.blur_tiles.clear(); P.fast_tiles.clear();
     for (int l = 0; l < ORB_LEVELS; l++) {
-        for (int y = 0; y < P.L.lv[l].h; y += BT_H) { P.blur_lvl.push_back(l); P.blur_y0.push_back(y); }
-        for (int y = 0; y < P.L.lv[l].h; y += FT_H) { P.fast_lvl.push_back(l); P.fast_y0.push_back(y); }
+        for (int y = 0; y < P.L.lv[l].h; y += BT_H) P.blur_tiles.push_back(tile_word(0, l, y));
+        for (int y = 0; y < P.L.lv[l].h; y += FT_H) P.fast_tiles.push_back(tile_word(0, l, y));
     }
+}
+
+// The images of one call: host images (staged in pinned memory and uploaded here, all of one size) or B,G,R images that are already on
+// the device (packed rows, any sizes).
+struct OrbInput {
+    const uint8_t* const* host = nullptr; int channels = 3; size_t row_stride = 0;
+    const uint8_t* const* dev = nullptr;
+};
+
+// One group of images: the layouts of its slots with their arena offsets, its tables and the sizes of its arenas.
+struct OrbGroup {
+    int i0 = 0, nb = 0;                                   // first image of the call, images
+    std::vector<OrbLayout> L;
+    std::vector<int32_t> taps;                            // the taps of every distinct size of the group, once
+    std::vector<uint32_t> blur_tiles, fast_tiles;
+    std::vector<int> blur_at, fast_at;                    // first tile of every slot, then the total
+    std::vector<size_t> raw0, stage0;                     // slot's B,G,R upload in the raw arena / its host image in the pinned staging
+    size_t raw = 0, stage = 0, pix = 0, mask = 0, cnt = 0, cand = 0;    // bytes, bytes, bytes, mask words, row counters, candidates
+};
+
+void make_group(const std::vector<const OrbPlan*>& plan_of, int i0, int i1, const OrbInput& in, OrbGroup& G) {
+    G = OrbGroup{};
+    G.i0 = i0; G.nb = i1 - i0;
+    std::vector<std::pair<const OrbPlan*, int>> taps_at;
+    for (int s = 0; s < G.nb; s++) {
+        const OrbPlan& P = *plan_of[i0 + s];
+        int t0 = -1;
+        for (auto& pt : taps_at) if (pt.first == &P) t0 = pt.second;
+        if (t0 < 0) { t0 = (int)G.taps.size(); taps_at.emplace_back(&P, t0); G.taps.insert(G.taps.end(), P.taps.begin(), P.taps.end()); }
+        OrbLayout L = P.L;
+        for (int l = 0; l < ORB_LEVELS; l++) L.lv[l].taps += t0;
+        const size_t px = (size_t)L.lv[0].w * L.lv[0].h;
+        L.pix0 = G.pix; G.pix += (size_t)L.slab;
+        L.mask0 = G.mask; G.mask += (size_t)L.ncnt;
+        L.cnt0 = G.cnt; G.cnt += (size_t)L.total_rows + 1;
+        L.cand0 = G.cand; G.cand += (size_t)L.cand_cap;
+        L.src_stride = 3 * L.lv[0].w;
+        G.raw0.push_back(G.raw); G.raw += in.host && in.channels == 3 ? 3 * px : 0;
+        G.stage0.push_back(G.stage); G.stage += in.host ? px * in.channels : 0;
+        G.L.push_back(L);
+        G.blur_at.push_back((int)G.blur_tiles.size());
+        for (uint32_t t : P.blur_tiles) G.blur_tiles.push_back(t | (uint32_t)s << 16);
+        G.fast_at.push_back((int)G.fast_tiles.size());
+        for (uint32_t t : P.fast_tiles) G.fast_tiles.push_back(t | (uint32_t)s << 16);
+    }
+    G.blur_at.push_back((int)G.blur_tiles.size()); G.fast_at.push_back((int)G.fast_tiles.size());
+}
+
+// Device pointers of a group, carved in this order from ctx->orb_dev; the tables come first and mirror their pinned staging.
+struct OrbDev {
+    OrbLayout* L; int32_t* taps; uint32_t *blur_tiles, *fast_tiles;
+    uint8_t *raw, *pyr, *blur, *score; uint32_t* mask; int32_t *rowoff, *rowcnt, *lvl; uint2* cand;
+};
+size_t carve_tables(Carver& c, const OrbGroup& G, OrbDev& D) {
+    D.L = c.take<OrbLayout>(G.L.size());
+    D.taps = c.take<int32_t>(G.taps.size() + 4);
+    D.blur_tiles = c.take<uint32_t>(G.blur_tiles.size() + 4); D.fast_tiles = c.take<uint32_t>(G.fast_tiles.size() + 4);
+    return c.off;
+}
+size_t carve(Carver& c, const OrbGroup& G, OrbDev& D) {
+    carve_tables(c, G, D);
+    D.raw = c.take<uint8_t>(G.raw);
+    D.pyr = c.take<uint8_t>(G.pix); D.blur = c.take<uint8_t>(G.pix); D.score = c.take<uint8_t>(G.pix);
+    D.mask = c.take<uint32_t>(G.mask); D.rowoff = c.take<int32_t>(G.cnt); D.rowcnt = c.take<int32_t>(G.cnt);
+    D.lvl = c.take<int32_t>(16 * (size_t)G.nb);
+    D.cand = c.take<uint2>(G.cand);
+    return c.off;
 }
 
 inline double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-int orb_run(sfmb200_ctx* ctx, const uint8_t* const* images, int n_images, int w, int h, int channels, size_t row_stride, int nfeatures,
-            int cap, KeyPointOut* kp_out, uint8_t* desc_out, int32_t* n_out) {
-    OrbPlan P;
-    make_plan(w, h, nfeatures, P);
-    const OrbLayout& L = P.L;
-    if (L.total_rows > 65535 * BT_H) return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image too tall for one launch (%d pyramid rows)", L.total_rows);
+// Grey, pyramid, blur (side stream), FAST + suppression of slots [s0, s0 + n) of a group: no host involvement.
+int orb_detect(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, int s0, int n, bool grey_from_bgr) {
+    cudaStream_t st = ctx->stream;
+    int maxw = 0, maxh = 0, maxchunks = 0;
+    for (int s = s0; s < s0 + n; s++) {
+        maxw = std::max(maxw, G.L[s].lv[0].w); maxh = std::max(maxh, G.L[s].lv[0].h); maxchunks = std::max(maxchunks, G.L[s].chunks);
+    }
+    if (grey_from_bgr) {
+        orb_gray_kernel<<<dim3(ceil_div(maxw, 256), maxh, n), 256, 0, st>>>(D.L + s0, D.pyr);
+        SFM_LAUNCH_CHECK(ctx);
+    }
+    for (int l = 1; l < ORB_LEVELS; l++) {
+        int dw = 0, dh = 0;
+        for (int s = s0; s < s0 + n; s++) { dw = std::max(dw, G.L[s].lv[l].w); dh = std::max(dh, G.L[s].lv[l].h); }
+        if (dw == 0) break;
+        orb_resize_kernel<<<dim3(ceil_div(dw, 256), dh, n), 256, 0, st>>>(D.L + s0, D.pyr, l, D.taps);
+        SFM_LAUNCH_CHECK(ctx);
+    }
+    SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[0], st));
+    SFM_CUDA(ctx, cudaStreamWaitEvent(ctx->orb_stream, ctx->orb_ev[0], 0));
+    const int xb = ceil_div(maxw, BT_W);
+    const int64_t nbt = G.blur_at[s0 + n] - G.blur_at[s0], nft = G.fast_at[s0 + n] - G.fast_at[s0];
+    orb_blur_kernel<<<(unsigned)(nbt * xb), 256, 0, ctx->orb_stream>>>(D.pyr, D.blur, D.L, D.blur_tiles + G.blur_at[s0], xb);
+    SFM_LAUNCH_CHECK(ctx);
+    orb_fast_nms_kernel<<<(unsigned)(nft * maxchunks), dim3(FT_W, FT_TY), 0, st>>>(D.pyr, D.score, D.mask, D.rowcnt, D.L, D.fast_tiles + G.fast_at[s0], maxchunks);
+    SFM_LAUNCH_CHECK(ctx);
+    return SFMB200_OK;
+}
+
+// Input stage for host images: staging + upload, pipelined against detection.  The pool packs quarter images into pinned memory IN
+// IMAGE ORDER and every thread sends its piece off itself on the upload stream (a pageable cudaMemcpy would pack and copy serially on one
+// thread); whoever enqueues the last piece of an image records that image's event.  Detection runs per GROUP of images on the main
+// stream as soon as the group's images have landed, i.e. under the DMA of the following groups: the call is PCIe-bound.  Only worth it
+// for large batches (measured: 50 images 11.5 -> 9.9 ms, but 7 images 2.8 -> 3.5 ms -- 4x the launches on quarter-size grids and 28 small
+// copies): small batches send whole images and run detection once.
+int orb_input_host(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, const OrbInput& in) {
+    const int nb = G.nb, dev = ctx->device, channels = in.channels;
+    const bool pipelined = nb >= 16;
+    const int PIECES = pipelined ? 4 : 1;
+    while ((int)ctx->orb_img_ev.size() < nb) {
+        cudaEvent_t ev = nullptr;
+        SFM_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        ctx->orb_img_ev.push_back(ev);
+    }
+    std::unique_ptr<std::atomic<int>[]> pieces_done(new std::atomic<int>[nb]);
+    for (int s = 0; s < nb; s++) pieces_done[s].store(0);
+    std::atomic<int> task_err{0};
+    uint8_t* h_img = (uint8_t*)ctx->orb_pin_img.p;
+    cudaStream_t up = ctx->orb_up;
+    SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[0], ctx->stream));         // the previous group's kernels have read the buffers the uploads overwrite
+    SFM_CUDA(ctx, cudaStreamWaitEvent(up, ctx->orb_ev[0], 0));
+    ctx->pool->parallel_for(nb * PIECES, [&](int t) {
+        cudaSetDevice(dev);
+        const int s = t / PIECES, c = t % PIECES;
+        const OrbLayout& L = G.L[s];
+        const int w = L.lv[0].w, h = L.lv[0].h;
+        const int y0 = (int)((int64_t)h * c / PIECES), y1 = (int)((int64_t)h * (c + 1) / PIECES);
+        const size_t rb = (size_t)w * channels, off = (size_t)y0 * rb, bytes = (size_t)(y1 - y0) * rb;
+        uint8_t* dst = h_img + G.stage0[s] + off; const uint8_t* src = in.host[G.i0 + s] + (size_t)y0 * in.row_stride;
+        if (in.row_stride == rb) memcpy(dst, src, bytes);
+        else for (int y = 0; y < y1 - y0; y++) memcpy(dst + (size_t)y * rb, src + (size_t)y * in.row_stride, rb);
+        uint8_t* d = (channels == 1 ? D.pyr + L.pix0 : D.raw + G.raw0[s]) + off;
+        if (bytes && cudaMemcpyAsync(d, dst, bytes, cudaMemcpyHostToDevice, up) != cudaSuccess) task_err.store(1);
+        if (pieces_done[s].fetch_add(1) + 1 == PIECES && cudaEventRecord(ctx->orb_img_ev[s], up) != cudaSuccess) task_err.store(1);
+    });
+    if (task_err.load()) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    const int groups = pipelined ? 4 : 1, gsz = ceil_div(nb, groups);
+    for (int s0 = 0; s0 < nb; s0 += gsz) {
+        const int n = std::min(gsz, nb - s0);
+        for (int s = s0; s < s0 + n; s++) SFM_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->orb_img_ev[s], 0));
+        if (int rc = orb_detect(ctx, G, D, s0, n, channels == 3)) return rc;
+    }
+    return SFMB200_OK;
+}
+
+// The rest of the stage, whatever the input: ordered compaction, the three host round trips with the two retainBest selections,
+// describe, copy-out of the group's key points and descriptors.
+int orb_finish(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, int cap, KeyPointOut* kp_out, uint8_t* desc_out, int32_t* n_out,
+               std::vector<std::vector<Rec>>& task, double t0) {
+    cudaStream_t st = ctx->stream;
+    HostPool& pool = *ctx->pool;
+    double* tm = ctx->orb_ms;
+    const int nb = G.nb, i0 = G.i0;
+    int max_rows = 0;
+    for (const OrbLayout& L : G.L) max_rows = std::max(max_rows, L.total_rows);
+    SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[1], ctx->orb_stream));
+    orb_scan_kernel<<<nb, 1024, 0, st>>>(D.rowcnt, D.rowoff, D.lvl, D.L); SFM_LAUNCH_CHECK(ctx);
+    orb_scatter_kernel<<<dim3(ceil_div(max_rows * 32, 256), 1, nb), 256, 0, st>>>(D.mask, D.score, D.rowoff, D.L, D.cand);
+    SFM_LAUNCH_CHECK(ctx);
+    SFM_CUDA(ctx, ctx->orb_pin_a.reserve(64 * (size_t)nb + 64));
+    int32_t* h_lvl = (int32_t*)ctx->orb_pin_a.p;
+    SFM_CUDA(ctx, cudaMemcpyAsync(h_lvl, D.lvl, 64 * (size_t)nb, cudaMemcpyDeviceToHost, st));
+    double t1 = now_ms(); tm[0] += t1 - t0;
+    SFM_CUDA(ctx, cudaStreamSynchronize(st));
+    double t2 = now_ms(); tm[1] += t2 - t1;
+    // ---- round trip 1: candidates of every image (raster order per level)
+    std::vector<int32_t> lvl(h_lvl, h_lvl + 16 * (size_t)nb);
+    std::vector<size_t> cand_at(nb + 1, 0);
+    for (int s = 0; s < nb; s++) {
+        if (lvl[16 * s + ORB_LEVELS] > G.L[s].cand_cap) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "candidate buffer overflow (internal)");
+        cand_at[s + 1] = cand_at[s] + lvl[16 * s + ORB_LEVELS];
+    }
+    const size_t total_cand = cand_at[nb];
+    SFM_CUDA(ctx, ctx->orb_pin_b.reserve(8 * total_cand + 64));
+    uint2* h_cand = (uint2*)ctx->orb_pin_b.p;
+    for (int s = 0; s < nb; s++) {
+        const size_t n = cand_at[s + 1] - cand_at[s];
+        if (n) SFM_CUDA(ctx, cudaMemcpyAsync(h_cand + cand_at[s], D.cand + G.L[s].cand0, 8 * n, cudaMemcpyDeviceToHost, st));
+    }
+    SFM_CUDA(ctx, cudaStreamSynchronize(st));
+    double t3 = now_ms(); tm[2] += t3 - t2;
+    // ---- first selection: best 2 * quota FAST scores per (image, level); KeyPointsFilter::retainBest keeps ties
+    pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
+        const int s = t / ORB_LEVELS, l = t % ORB_LEVELS;
+        const int b = lvl[16 * s + l], e = lvl[16 * s + l + 1];
+        std::vector<Rec>& r = task[t];
+        r.resize(e - b);
+        const uint2* c = h_cand + cand_at[s];
+        for (int k = b; k < e; k++) r[k - b] = Rec{(float)(c[k].y & 0xFFFF), k};
+        retain_best(r, 2 * G.L[s].lv[l].quota);
+    });
+    std::vector<size_t> sel_at((size_t)nb * ORB_LEVELS + 1, 0);
+    for (int t = 0; t < nb * ORB_LEVELS; t++) sel_at[t + 1] = sel_at[t] + task[t].size();
+    const size_t nsel = sel_at[(size_t)nb * ORB_LEVELS];
+    SFM_CUDA(ctx, ctx->orb_pin_c.reserve(Carver::pad(8 * nsel + 16) * 2 + Carver::pad(4 * nsel + 16) * 2 + 1024));
+    Carver pc(ctx->orb_pin_c.p);
+    uint2* h_sel = pc.take<uint2>(nsel + 2); float* h_resp = pc.take<float>(nsel + 4);
+    uint2* h_fin = pc.take<uint2>(nsel + 2); float* h_fresp = pc.take<float>(nsel + 4);
+    pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
+        const int s = t / ORB_LEVELS, l = t % ORB_LEVELS;
+        const uint2* c = h_cand + cand_at[s];
+        uint2* o = h_sel + sel_at[t];
+        for (const Rec& r : task[t]) *o++ = make_uint2(c[r.idx].x, (unsigned)l | ((unsigned)s << 8));
+    });
+    SFM_CUDA(ctx, ctx->orb_lists.reserve(Carver::pad(8 * nsel + 16) * 2 + Carver::pad(4 * nsel + 16) * 2 + Carver::pad(28 * nsel + 32) + Carver::pad(32 * nsel + 32) + 4096));
+    Carver lc(ctx->orb_lists.p);
+    uint2* d_sel = lc.take<uint2>(nsel + 2); float* d_resp = lc.take<float>(nsel + 4);
+    uint2* d_fin = lc.take<uint2>(nsel + 2); float* d_fresp = lc.take<float>(nsel + 4);
+    KeyPointOut* d_kp = lc.take<KeyPointOut>(nsel + 1); uint8_t* d_desc = lc.take<uint8_t>(32 * nsel + 32);
+    double t4 = now_ms(); tm[3] += t4 - t3;
+    if (nsel) {
+        SFM_CUDA(ctx, cudaMemcpyAsync(d_sel, h_sel, 8 * nsel, cudaMemcpyHostToDevice, st));
+        orb_harris_kernel<<<(unsigned)ceil_div64((int64_t)nsel * 32, 256), 256, 0, st>>>(D.pyr, D.L, d_sel, (int)nsel, d_resp);
+        SFM_LAUNCH_CHECK(ctx);
+        SFM_CUDA(ctx, cudaMemcpyAsync(h_resp, d_resp, 4 * nsel, cudaMemcpyDeviceToHost, st));
+        SFM_CUDA(ctx, cudaStreamSynchronize(st));                                              // round trip 2
+    }
+    double t5 = now_ms(); tm[4] += t5 - t4;
+    // ---- second selection: best quota Harris responses per (image, level)
+    pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
+        const int s = t / ORB_LEVELS, l = t % ORB_LEVELS;
+        const int n = (int)(sel_at[t + 1] - sel_at[t]);
+        std::vector<Rec>& r = task[t];
+        r.resize(n);
+        const float* rs = h_resp + sel_at[t];
+        for (int k = 0; k < n; k++) r[k] = Rec{rs[k], k};
+        retain_best(r, G.L[s].lv[l].quota);
+    });
+    std::vector<size_t> fin_at((size_t)nb * ORB_LEVELS + 1, 0);
+    for (int t = 0; t < nb * ORB_LEVELS; t++) fin_at[t + 1] = fin_at[t] + task[t].size();
+    const size_t nfin = fin_at[(size_t)nb * ORB_LEVELS];
+    pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
+        uint2* o = h_fin + fin_at[t]; float* f = h_fresp + fin_at[t];
+        const uint2* src = h_sel + sel_at[t];
+        for (const Rec& r : task[t]) { *o++ = src[r.idx]; *f++ = r.response; }
+    });
+    double t6 = now_ms(); tm[5] += t6 - t5;
+    if (nfin) {
+        SFM_CUDA(ctx, ctx->orb_pin_a.reserve((28 + 32) * nfin + 256));
+        KeyPointOut* h_kp = (KeyPointOut*)ctx->orb_pin_a.p; uint8_t* h_desc = (uint8_t*)(h_kp + nfin);
+        SFM_CUDA(ctx, cudaMemcpyAsync(d_fin, h_fin, 8 * nfin, cudaMemcpyHostToDevice, st));
+        SFM_CUDA(ctx, cudaMemcpyAsync(d_fresp, h_fresp, 4 * nfin, cudaMemcpyHostToDevice, st));
+        SFM_CUDA(ctx, cudaStreamWaitEvent(st, ctx->orb_ev[1], 0));
+        orb_describe_kernel<<<(unsigned)ceil_div64((int64_t)nfin * 32, 256), 256, 0, st>>>(D.pyr, D.blur, D.L, d_fin, d_fresp, (int)nfin, d_kp, d_desc);
+        SFM_LAUNCH_CHECK(ctx);
+        SFM_CUDA(ctx, cudaMemcpyAsync(h_kp, d_kp, 28 * nfin, cudaMemcpyDeviceToHost, st));
+        SFM_CUDA(ctx, cudaMemcpyAsync(h_desc, d_desc, 32 * nfin, cudaMemcpyDeviceToHost, st));
+        SFM_CUDA(ctx, cudaStreamSynchronize(st));                                              // round trip 3
+        double t7 = now_ms(); tm[6] += t7 - t6;
+        pool.parallel_for(nb, [&](int s) {
+            const size_t at = fin_at[(size_t)s * ORB_LEVELS], n_all = fin_at[(size_t)(s + 1) * ORB_LEVELS] - at;
+            const size_t n = std::min<size_t>(n_all, (size_t)cap);
+            if (n) {
+                memcpy(kp_out + (size_t)(i0 + s) * cap, h_kp + at, 28 * n);
+                memcpy(desc_out + (size_t)(i0 + s) * cap * 32, h_desc + 32 * at, 32 * n);
+            }
+        });
+        tm[7] += now_ms() - t7;
+    }
+    for (int s = 0; s < nb; s++) n_out[i0 + s] = (int32_t)(fin_at[(size_t)(s + 1) * ORB_LEVELS] - fin_at[(size_t)s * ORB_LEVELS]);
+    SFM_CUDA(ctx, cudaStreamSynchronize(ctx->orb_stream));        // the next group (and a download for inspection) reuses the blur buffer
+    return SFMB200_OK;
+}
+
+// n_images images of sizes ws[i] x hs[i] from `in`: one plan per distinct size, groups by device bytes (orb_groups.h), and per group the
+// input stage, then the shared rest.
+int orb_run(sfmb200_ctx* ctx, const OrbInput& in, int n_images, const int* ws, const int* hs, int nfeatures, int cap, KeyPointOut* kp_out,
+            uint8_t* desc_out, int32_t* n_out) {
+    const bool host = in.host != nullptr;
+    std::map<std::pair<int, int>, OrbPlan> plans;
+    std::vector<const OrbPlan*> plan_of(n_images);
+    std::vector<size_t> dev_bytes(n_images), stage_bytes(n_images);
+    for (int i = 0; i < n_images; i++) {
+        auto it = plans.find({ws[i], hs[i]});
+        if (it == plans.end()) {
+            it = plans.emplace(std::make_pair(ws[i], hs[i]), OrbPlan{}).first;
+            make_plan(ws[i], hs[i], nfeatures, it->second);
+            if (it->second.L.total_rows > 65535 * BT_H)
+                return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image too tall for one launch (%d pyramid rows)", it->second.L.total_rows);
+        }
+        plan_of[i] = &it->second;
+        const size_t img_bytes = (size_t)ws[i] * hs[i] * (host ? in.channels : 3);
+        dev_bytes[i] = orb_image_bytes(it->second.L, host && in.channels == 3 ? img_bytes : 0);
+        stage_bytes[i] = host ? img_bytes : 0;
+    }
+    const std::vector<int> gstart = orb_groups(dev_bytes.data(), host ? stage_bytes.data() : nullptr, n_images);
+    const int ngroups = (int)gstart.size() - 1;
+    std::vector<OrbGroup> groups(ngroups);
+    size_t dev_need = 0, tab_need = 0, stage_need = 0;
+    int max_nb = 0;
+    for (int g = 0; g < ngroups; g++) {
+        OrbGroup& G = groups[g];
+        make_group(plan_of, gstart[g], gstart[g + 1], in, G);
+        OrbDev D;
+        Carver a(nullptr), b(nullptr);
+        dev_need = std::max(dev_need, carve(a, G, D));
+        tab_need = std::max(tab_need, carve_tables(b, G, D));
+        stage_need = std::max(stage_need, G.stage);
+        max_nb = std::max(max_nb, G.nb);
+    }
     cudaStream_t st = ctx->stream;
     if (!ctx->orb_stream) {
         SFM_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->orb_stream, cudaStreamNonBlocking));
@@ -417,213 +698,51 @@ int orb_run(sfmb200_ctx* ctx, const uint8_t* const* images, int n_images, int w,
         for (auto& ev : ctx->orb_ev) SFM_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     }
     if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
-    HostPool& pool = *ctx->pool;
     double* tm = ctx->orb_ms;
     for (int i = 0; i < 8; i++) tm[i] = 0.0;
-
-    const size_t img_bytes = (size_t)w * h * channels;
-    const size_t raw_img = channels == 3 ? img_bytes : 0;
-    const int cand_cap = L.slab / 4 + 64;                    // 3x3 non-maximum suppression keeps at most one pixel of every 2x2 block
-    const size_t per_img = Carver::pad(raw_img) + 3 * Carver::pad(L.slab) + Carver::pad(4 * (size_t)L.ncnt) + 2 * Carver::pad(4 * (size_t)(L.total_rows + 1)) +
-                           Carver::pad(64) + Carver::pad(8 * (size_t)cand_cap);
-    // a batch = as many images as 2 GB of device scratch and 96 MB of pinned staging hold
-    const int slots = (int)std::max<size_t>(1, std::min<size_t>({(size_t)n_images, ((size_t)2 << 30) / per_img, ((size_t)96 << 20) / img_bytes}));
-    const size_t fixed = Carver::pad(4 * P.taps.size() + 16) + 4 * Carver::pad(4 * P.fast_lvl.size() + 16) + 4096;
-    SFM_CUDA(ctx, ctx->orb_dev.reserve(fixed + per_img * slots + (size_t)slots * 2048));
-    Carver cv(ctx->orb_dev.p);
-    int32_t* d_taps = cv.take<int32_t>(P.taps.size() + 4);
-    int32_t* d_blur_lvl = cv.take<int32_t>(P.blur_lvl.size() + 4); int32_t* d_blur_y0 = cv.take<int32_t>(P.blur_y0.size() + 4);
-    int32_t* d_fast_lvl = cv.take<int32_t>(P.fast_lvl.size() + 4); int32_t* d_fast_y0 = cv.take<int32_t>(P.fast_y0.size() + 4);
-    uint8_t* d_raw = cv.take<uint8_t>(raw_img * slots);
-    uint8_t* d_pyr = cv.take<uint8_t>((size_t)L.slab * slots); uint8_t* d_blur = cv.take<uint8_t>((size_t)L.slab * slots);
-    uint8_t* d_score = cv.take<uint8_t>((size_t)L.slab * slots);
-    uint32_t* d_mask = cv.take<uint32_t>((size_t)L.ncnt * slots); int32_t* d_rowoff = cv.take<int32_t>((size_t)(L.total_rows + 1) * slots);
-    int32_t* d_rowcnt = cv.take<int32_t>((size_t)(L.total_rows + 1) * slots);
-    int32_t* d_lvl = cv.take<int32_t>(16 * (size_t)slots);
-    uint2* d_cand = cv.take<uint2>((size_t)cand_cap * slots);
-    ctx->orb_last = OrbLast{d_pyr, d_blur, d_score, L.slab, 0, w, h, nfeatures};
-    if (!P.taps.empty()) SFM_CUDA(ctx, cudaMemcpyAsync(d_taps, P.taps.data(), 4 * P.taps.size(), cudaMemcpyHostToDevice, st));
-    SFM_CUDA(ctx, cudaMemcpyAsync(d_blur_lvl, P.blur_lvl.data(), 4 * P.blur_lvl.size(), cudaMemcpyHostToDevice, st));
-    SFM_CUDA(ctx, cudaMemcpyAsync(d_blur_y0, P.blur_y0.data(), 4 * P.blur_y0.size(), cudaMemcpyHostToDevice, st));
-    SFM_CUDA(ctx, cudaMemcpyAsync(d_fast_lvl, P.fast_lvl.data(), 4 * P.fast_lvl.size(), cudaMemcpyHostToDevice, st));
-    SFM_CUDA(ctx, cudaMemcpyAsync(d_fast_y0, P.fast_y0.data(), 4 * P.fast_y0.size(), cudaMemcpyHostToDevice, st));
-    SFM_CUDA(ctx, ctx->orb_pin_img.reserve(img_bytes * slots + 256));
-    uint8_t* h_img = (uint8_t*)ctx->orb_pin_img.p;
-
-    std::vector<std::vector<Rec>> task((size_t)slots * ORB_LEVELS);
-    std::atomic<int> task_err{0};
-    for (int i0 = 0; i0 < n_images; i0 += slots) {
-        const int nb = std::min(slots, n_images - i0);
-        double t0 = now_ms();
-        // ---- staging + upload, pipelined against detection.  The pool packs quarter images into pinned memory IN IMAGE ORDER and every
-        //      thread sends its piece off itself on the upload stream (a pageable cudaMemcpy would pack and copy serially on one thread);
-        //      whoever enqueues the last piece of an image records that image's event.  Detection runs per GROUP of images on the
-        //      main stream as soon as the group's images have landed, i.e. under the DMA of the following groups: the call is PCIe-bound.
-        //      Only worth it for large batches (measured: 50 images 11.5 -> 9.9 ms, but 7 images 2.8 -> 3.5 ms -- 4x the launches on
-        //      quarter-size grids and 28 small copies): small batches send whole images and run detection once.
-        const int dev = ctx->device;
-        const bool pipelined = nb >= 16;
-        const int PIECES = pipelined ? 4 : 1;
-        while ((int)ctx->orb_img_ev.size() < nb) {
-            cudaEvent_t ev = nullptr;
-            SFM_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-            ctx->orb_img_ev.push_back(ev);
+    SFM_CUDA(ctx, ctx->orb_dev.reserve(dev_need + 4096));
+    SFM_CUDA(ctx, ctx->orb_pin_tab.reserve(tab_need + 256));
+    if (host) SFM_CUDA(ctx, ctx->orb_pin_img.reserve(stage_need + 256));
+    std::vector<std::vector<Rec>> task((size_t)max_nb * ORB_LEVELS);
+    for (OrbGroup& G : groups) {
+        const double t0 = now_ms();
+        OrbDev D;
+        Carver cv(ctx->orb_dev.p);
+        carve(cv, G, D);
+        for (int s = 0; s < G.nb; s++) {
+            OrbLayout& L = G.L[s];
+            L.src = host ? (in.channels == 3 ? D.raw + G.raw0[s] : nullptr) : in.dev[G.i0 + s];
         }
-        std::unique_ptr<std::atomic<int>[]> pieces_done(new std::atomic<int>[nb]);
-        for (int s = 0; s < nb; s++) pieces_done[s].store(0);
-        cudaStream_t up = ctx->orb_up;
-        SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[0], st));                 // the previous batch's kernels have read the buffers the uploads overwrite
-        SFM_CUDA(ctx, cudaStreamWaitEvent(up, ctx->orb_ev[0], 0));
-        pool.parallel_for(nb * PIECES, [&](int t) {
-            cudaSetDevice(dev);
-            const int s = t / PIECES, c = t % PIECES;
-            const int y0 = (int)((int64_t)h * c / PIECES), y1 = (int)((int64_t)h * (c + 1) / PIECES);
-            const size_t rb = (size_t)w * channels, off = (size_t)y0 * rb, bytes = (size_t)(y1 - y0) * rb;
-            uint8_t* dst = h_img + (size_t)s * img_bytes + off; const uint8_t* src = images[i0 + s] + (size_t)y0 * row_stride;
-            if (row_stride == rb) memcpy(dst, src, bytes);
-            else for (int y = 0; y < y1 - y0; y++) memcpy(dst + (size_t)y * rb, src + (size_t)y * row_stride, rb);
-            uint8_t* d = (channels == 1 ? d_pyr + (size_t)s * L.slab : d_raw + (size_t)s * raw_img) + off;
-            if (bytes && cudaMemcpyAsync(d, dst, bytes, cudaMemcpyHostToDevice, up) != cudaSuccess) task_err.store(1);
-            if (pieces_done[s].fetch_add(1) + 1 == PIECES && cudaEventRecord(ctx->orb_img_ev[s], up) != cudaSuccess) task_err.store(1);
-        });
-        if (task_err.load()) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-        // ---- grey, pyramid, blur (side stream), FAST + suppression per group; ordered compaction for the whole batch: no host involvement
-        SFM_CUDA(ctx, cudaMemsetAsync(d_rowcnt, 0, 4 * (size_t)(L.total_rows + 1) * nb, st));
-        const int groups = pipelined ? 4 : 1, gsz = ceil_div(nb, groups);
-        for (int s0 = 0; s0 < nb; s0 += gsz) {
-            const int n = std::min(gsz, nb - s0);
-            for (int s = s0; s < s0 + n; s++) SFM_CUDA(ctx, cudaStreamWaitEvent(st, ctx->orb_img_ev[s], 0));
-            uint8_t* g_pyr = d_pyr + (size_t)s0 * L.slab;
-            if (channels == 3) {
-                orb_gray_kernel<<<dim3(ceil_div(w, 256), h, n), 256, 0, st>>>(d_raw + (size_t)s0 * raw_img, raw_img, 3 * w, w, h, g_pyr, L.slab);
-                SFM_LAUNCH_CHECK(ctx);
-            }
-            for (int l = 1; l < ORB_LEVELS; l++) {
-                const OrbLevel& d = L.lv[l]; const OrbLevel& sl = L.lv[l - 1];
-                if (d.w == 0) break;
-                orb_resize_kernel<<<dim3(ceil_div(d.w, 256), d.h, n), 256, 0, st>>>(g_pyr, L.slab, sl.off, sl.w, d.off, d.w, d.h, d_taps + P.taps_off[l]);
-                SFM_LAUNCH_CHECK(ctx);
-            }
-            SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[0], st));
-            SFM_CUDA(ctx, cudaStreamWaitEvent(ctx->orb_stream, ctx->orb_ev[0], 0));
-            orb_blur_kernel<<<dim3(ceil_div(w, BT_W), (unsigned)P.blur_lvl.size(), n), 256, 0, ctx->orb_stream>>>(g_pyr, d_blur + (size_t)s0 * L.slab, L, d_blur_lvl, d_blur_y0);
-            SFM_LAUNCH_CHECK(ctx);
-            orb_fast_nms_kernel<<<dim3(L.chunks, (unsigned)P.fast_lvl.size(), n), dim3(FT_W, FT_TY), 0, st>>>(
-                g_pyr, d_score + (size_t)s0 * L.slab, d_mask + (size_t)s0 * L.ncnt, d_rowcnt + (size_t)s0 * (L.total_rows + 1), L, d_fast_lvl, d_fast_y0);
-            SFM_LAUNCH_CHECK(ctx);
-        }
-        SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[1], ctx->orb_stream));
-        orb_scan_kernel<<<nb, 1024, 0, st>>>(d_rowcnt, d_rowoff, d_lvl, L); SFM_LAUNCH_CHECK(ctx);
-        orb_scatter_kernel<<<dim3(ceil_div(L.total_rows * 32, 256), 1, nb), 256, 0, st>>>(d_mask, d_score, d_rowoff, L, d_cand, cand_cap);
-        SFM_LAUNCH_CHECK(ctx);
-        SFM_CUDA(ctx, ctx->orb_pin_a.reserve(64 * (size_t)nb + 64));
-        int32_t* h_lvl = (int32_t*)ctx->orb_pin_a.p;
-        SFM_CUDA(ctx, cudaMemcpyAsync(h_lvl, d_lvl, 64 * (size_t)nb, cudaMemcpyDeviceToHost, st));
-        double t1 = now_ms(); tm[0] += t1 - t0;
-        SFM_CUDA(ctx, cudaStreamSynchronize(st));
-        ctx->orb_last.nimg = nb;
-        double t2 = now_ms(); tm[1] += t2 - t1;
-        // ---- round trip 1: candidates of every image (raster order per level)
-        std::vector<int32_t> lvl(h_lvl, h_lvl + 16 * (size_t)nb);
-        std::vector<size_t> cand_at(nb + 1, 0);
-        for (int s = 0; s < nb; s++) {
-            if (lvl[16 * s + ORB_LEVELS] > cand_cap) return sfmb200_fail(ctx, SFMB200_ERR_CUDA, "candidate buffer overflow (internal)");
-            cand_at[s + 1] = cand_at[s] + lvl[16 * s + ORB_LEVELS];
-        }
-        const size_t total_cand = cand_at[nb];
-        SFM_CUDA(ctx, ctx->orb_pin_b.reserve(8 * total_cand + 64));
-        uint2* h_cand = (uint2*)ctx->orb_pin_b.p;
-        for (int s = 0; s < nb; s++) {
-            const size_t n = cand_at[s + 1] - cand_at[s];
-            if (n) SFM_CUDA(ctx, cudaMemcpyAsync(h_cand + cand_at[s], d_cand + (size_t)s * cand_cap, 8 * n, cudaMemcpyDeviceToHost, st));
-        }
-        SFM_CUDA(ctx, cudaStreamSynchronize(st));
-        double t3 = now_ms(); tm[2] += t3 - t2;
-        // ---- first selection: best 2 * quota FAST scores per (image, level); KeyPointsFilter::retainBest keeps ties
-        pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
-            const int s = t / ORB_LEVELS, l = t % ORB_LEVELS;
-            const int b = lvl[16 * s + l], e = lvl[16 * s + l + 1];
-            std::vector<Rec>& r = task[t];
-            r.resize(e - b);
-            const uint2* c = h_cand + cand_at[s];
-            for (int k = b; k < e; k++) r[k - b] = Rec{(float)(c[k].y & 0xFFFF), k};
-            retain_best(r, 2 * L.lv[l].quota);
-        });
-        std::vector<size_t> sel_at((size_t)nb * ORB_LEVELS + 1, 0);
-        for (int t = 0; t < nb * ORB_LEVELS; t++) sel_at[t + 1] = sel_at[t] + task[t].size();
-        const size_t nsel = sel_at[(size_t)nb * ORB_LEVELS];
-        SFM_CUDA(ctx, ctx->orb_pin_c.reserve(Carver::pad(8 * nsel + 16) * 2 + Carver::pad(4 * nsel + 16) * 2 + 1024));
-        Carver pc(ctx->orb_pin_c.p);
-        uint2* h_sel = pc.take<uint2>(nsel + 2); float* h_resp = pc.take<float>(nsel + 4);
-        uint2* h_fin = pc.take<uint2>(nsel + 2); float* h_fresp = pc.take<float>(nsel + 4);
-        pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
-            const int s = t / ORB_LEVELS, l = t % ORB_LEVELS;
-            const uint2* c = h_cand + cand_at[s];
-            uint2* o = h_sel + sel_at[t];
-            for (const Rec& r : task[t]) *o++ = make_uint2(c[r.idx].x, (unsigned)l | ((unsigned)s << 8));
-        });
-        SFM_CUDA(ctx, ctx->orb_lists.reserve(Carver::pad(8 * nsel + 16) * 2 + Carver::pad(4 * nsel + 16) * 2 + Carver::pad(28 * nsel + 32) + Carver::pad(32 * nsel + 32) + 4096));
-        Carver lc(ctx->orb_lists.p);
-        uint2* d_sel = lc.take<uint2>(nsel + 2); float* d_resp = lc.take<float>(nsel + 4);
-        uint2* d_fin = lc.take<uint2>(nsel + 2); float* d_fresp = lc.take<float>(nsel + 4);
-        KeyPointOut* d_kp = lc.take<KeyPointOut>(nsel + 1); uint8_t* d_desc = lc.take<uint8_t>(32 * nsel + 32);
-        double t4 = now_ms(); tm[3] += t4 - t3;
-        if (nsel) {
-            SFM_CUDA(ctx, cudaMemcpyAsync(d_sel, h_sel, 8 * nsel, cudaMemcpyHostToDevice, st));
-            orb_harris_kernel<<<(unsigned)ceil_div64((int64_t)nsel * 32, 256), 256, 0, st>>>(d_pyr, L, d_sel, (int)nsel, d_resp);
-            SFM_LAUNCH_CHECK(ctx);
-            SFM_CUDA(ctx, cudaMemcpyAsync(h_resp, d_resp, 4 * nsel, cudaMemcpyDeviceToHost, st));
-            SFM_CUDA(ctx, cudaStreamSynchronize(st));                                              // round trip 2
-        }
-        double t5 = now_ms(); tm[4] += t5 - t4;
-        // ---- second selection: best quota Harris responses per (image, level)
-        pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
-            const int l = t % ORB_LEVELS;
-            const int n = (int)(sel_at[t + 1] - sel_at[t]);
-            std::vector<Rec>& r = task[t];
-            r.resize(n);
-            const float* rs = h_resp + sel_at[t];
-            for (int k = 0; k < n; k++) r[k] = Rec{rs[k], k};
-            retain_best(r, L.lv[l].quota);
-        });
-        std::vector<size_t> fin_at((size_t)nb * ORB_LEVELS + 1, 0);
-        for (int t = 0; t < nb * ORB_LEVELS; t++) fin_at[t + 1] = fin_at[t] + task[t].size();
-        const size_t nfin = fin_at[(size_t)nb * ORB_LEVELS];
-        pool.parallel_for(nb * ORB_LEVELS, [&](int t) {
-            uint2* o = h_fin + fin_at[t]; float* f = h_fresp + fin_at[t];
-            const uint2* src = h_sel + sel_at[t];
-            for (const Rec& r : task[t]) { *o++ = src[r.idx]; *f++ = r.response; }
-        });
-        double t6 = now_ms(); tm[5] += t6 - t5;
-        if (nfin) {
-            SFM_CUDA(ctx, ctx->orb_pin_a.reserve((28 + 32) * nfin + 256));
-            KeyPointOut* h_kp = (KeyPointOut*)ctx->orb_pin_a.p; uint8_t* h_desc = (uint8_t*)(h_kp + nfin);
-            SFM_CUDA(ctx, cudaMemcpyAsync(d_fin, h_fin, 8 * nfin, cudaMemcpyHostToDevice, st));
-            SFM_CUDA(ctx, cudaMemcpyAsync(d_fresp, h_fresp, 4 * nfin, cudaMemcpyHostToDevice, st));
-            SFM_CUDA(ctx, cudaStreamWaitEvent(st, ctx->orb_ev[1], 0));
-            orb_describe_kernel<<<(unsigned)ceil_div64((int64_t)nfin * 32, 256), 256, 0, st>>>(d_pyr, d_blur, L, d_fin, d_fresp, (int)nfin, d_kp, d_desc);
-            SFM_LAUNCH_CHECK(ctx);
-            SFM_CUDA(ctx, cudaMemcpyAsync(h_kp, d_kp, 28 * nfin, cudaMemcpyDeviceToHost, st));
-            SFM_CUDA(ctx, cudaMemcpyAsync(h_desc, d_desc, 32 * nfin, cudaMemcpyDeviceToHost, st));
-            SFM_CUDA(ctx, cudaStreamSynchronize(st));                                              // round trip 3
-            double t7 = now_ms(); tm[6] += t7 - t6;
-            pool.parallel_for(nb, [&](int s) {
-                const size_t at = fin_at[(size_t)s * ORB_LEVELS], n_all = fin_at[(size_t)(s + 1) * ORB_LEVELS] - at;
-                const size_t n = std::min<size_t>(n_all, (size_t)cap);
-                if (n) {
-                    memcpy(kp_out + (size_t)(i0 + s) * cap, h_kp + at, 28 * n);
-                    memcpy(desc_out + (size_t)(i0 + s) * cap * 32, h_desc + 32 * at, 32 * n);
-                }
-            });
-            tm[7] += now_ms() - t7;
-        }
-        for (int s = 0; s < nb; s++) n_out[i0 + s] = (int32_t)(fin_at[(size_t)(s + 1) * ORB_LEVELS] - fin_at[(size_t)s * ORB_LEVELS]);
-        SFM_CUDA(ctx, cudaStreamSynchronize(ctx->orb_stream));        // the next batch (and a download for inspection) reuses the blur buffer
+        // the tables: packed into pinned memory with the device carve's offsets, one upload
+        Carver tc(ctx->orb_pin_tab.p);
+        OrbDev H;
+        const size_t tab_bytes = carve_tables(tc, G, H);
+        memcpy(H.L, G.L.data(), sizeof(OrbLayout) * G.L.size());
+        if (!G.taps.empty()) memcpy(H.taps, G.taps.data(), 4 * G.taps.size());
+        memcpy(H.blur_tiles, G.blur_tiles.data(), 4 * G.blur_tiles.size());
+        memcpy(H.fast_tiles, G.fast_tiles.data(), 4 * G.fast_tiles.size());
+        SFM_CUDA(ctx, cudaMemcpyAsync(ctx->orb_dev.p, ctx->orb_pin_tab.p, tab_bytes, cudaMemcpyHostToDevice, st));
+        SFM_CUDA(ctx, cudaMemsetAsync(D.rowcnt, 0, 4 * G.cnt, st));
+        OrbLast& o = ctx->orb_last;
+        o.pyr = D.pyr; o.blur = D.blur; o.score = D.score; o.nimg = 0; o.nfeatures = nfeatures;
+        o.w.clear(); o.h.clear(); o.pix0.clear();
+        for (const OrbLayout& L : G.L) { o.w.push_back(L.lv[0].w); o.h.push_back(L.lv[0].h); o.pix0.push_back(L.pix0); }
+        if (int rc = host ? orb_input_host(ctx, G, D, in) : orb_detect(ctx, G, D, 0, G.nb, true)) return rc;
+        o.nimg = G.nb;
+        if (int rc = orb_finish(ctx, G, D, cap, kp_out, desc_out, n_out, task, t0)) return rc;
     }
     return SFMB200_OK;
 }
 
 }  // namespace
+
+// The images of sfmb200_decode_jpeg_extract_orb (jpeg.cu), already on the device: packed B,G,R rows of ws[i] x hs[i] pixels at d_bgr[i].
+int orb_extract_device(sfmb200_ctx* ctx, const uint8_t* const* d_bgr, const int* ws, const int* hs, int n, int nfeatures, int max_keypoints,
+                       sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints) {
+    OrbInput in;
+    in.dev = d_bgr;
+    return orb_run(ctx, in, n, ws, hs, nfeatures, max_keypoints, (KeyPointOut*)keypoints, descriptors, n_keypoints);
+}
 
 extern "C" {
 
@@ -645,7 +764,10 @@ int sfmb200_orb_detect_and_compute_batch(sfmb200_ctx* ctx, const uint8_t* const*
     for (int i = 0; i < n_images; i++) if (!images[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d is NULL", i);
     std::lock_guard<std::mutex> lk(ctx->mu);
     SFM_CUDA(ctx, cudaSetDevice(ctx->device));
-    return orb_run(ctx, images, n_images, width, height, channels, row_stride, nfeatures, max_keypoints, (KeyPointOut*)keypoints, descriptors, n_keypoints);
+    OrbInput in;
+    in.host = images; in.channels = channels; in.row_stride = row_stride;
+    const std::vector<int> ws(n_images, width), hs(n_images, height);
+    return orb_run(ctx, in, n_images, ws.data(), hs.data(), nfeatures, max_keypoints, (KeyPointOut*)keypoints, descriptors, n_keypoints);
 }
 
 int sfmb200_orb_detect_and_compute(sfmb200_ctx* ctx, const uint8_t* image, int width, int height, int channels, size_t row_stride, int nfeatures,
@@ -705,12 +827,12 @@ int sfmb200_orb_download_level(sfmb200_ctx* ctx, int stage, int image, int level
     std::lock_guard<std::mutex> lk(ctx->mu);
     const OrbLast& o = ctx->orb_last;
     if (!o.pyr || image < 0 || image >= o.nimg) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "no extraction to inspect (image %d of %d)", image, o.nimg);
-    OrbLayout L; make_layout(o.w, o.h, o.nfeatures, L);
+    OrbLayout L; make_layout(o.w[image], o.h[image], o.nfeatures, L);
     const uint8_t* base = stage == 0 ? o.pyr : stage == 1 ? o.blur : stage == 2 ? o.score : nullptr;
     if (!base) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "stage must be 0 (pyramid), 1 (blurred) or 2 (FAST score)");
     SFM_CUDA(ctx, cudaSetDevice(ctx->device));
     if (L.lv[level].w == 0) return SFMB200_OK;
-    SFM_CUDA(ctx, cudaMemcpyAsync(out, base + (size_t)image * o.slab + L.lv[level].off, (size_t)L.lv[level].w * L.lv[level].h, cudaMemcpyDeviceToHost, ctx->stream));
+    SFM_CUDA(ctx, cudaMemcpyAsync(out, base + o.pix0[image] + L.lv[level].off, (size_t)L.lv[level].w * L.lv[level].h, cudaMemcpyDeviceToHost, ctx->stream));
     SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SFMB200_OK;
 }

@@ -22,4 +22,11 @@ namespace sfmtoylib {
 // `images` unchanged) on any failure, including a factor cv::resize would refuse.
 bool readImages(const std::vector<std::string>& filenames, std::vector<cv::Mat>& images, float downscale = 1.0f);
 
+// readImages followed by SfM::extractFeatures (SfM.cpp:141-154) on every image, in one call (sfmb200_decode_jpeg_extract_orb): the
+// images stay on the device between the decode and ORB(5000), and may differ in size.  Appends to `images` as readImages does and
+// one Features per image to `features`, filled as SfM2DFeatureUtilities::extractFeatures fills them (keyPoints, descriptors, points).
+// false (and both vectors unchanged) on any failure.
+bool readImagesAndFeatures(const std::vector<std::string>& filenames, std::vector<cv::Mat>& images, std::vector<Features>& features,
+                           float downscale = 1.0f);
+
 }  // namespace sfmtoylib

@@ -15,6 +15,7 @@
 #endif
 #endif
 #include "../../include/sfmb200.h"
+#include "sfm_features.h"
 
 #include <cstdio>
 #include <cstring>
@@ -47,11 +48,6 @@ void check(int rc, const char* what) {
     }
 }
 
-#if defined(SFMB200_WITH_REFERENCE_HEADERS) || defined(SFMB200_WITH_OPENCV)
-const int kType8U = CV_8U;                    // OpenCV's macro
-#else
-const int kType8U = cv::CV_8U;                // cv_min.h
-#endif
 const double kNNMatchRatio = 0.8f;            // NN_MATCH_RATIO: the float literal widened to double
 const float kMaxReprojectionError = 10.0f;    // MIN_REPROJECTION_ERROR
 #if defined(SFMB200_SHIM_POSE) && !defined(SFMB200_WITH_REFERENCE_HEADERS)
@@ -71,9 +67,7 @@ SfM2DFeatureUtilities::~SfM2DFeatureUtilities() {}
 // SfM2DFeatureUtilities.cpp:46-51: mDetector->detectAndCompute(image, noArray(), keyPoints, descriptors) with ORB::create(5000),
 // then KeyPointsToPoints.  `image` is what cv::imread returned (8-bit B,G,R; SfM.cpp:124) or an 8-bit grey image.
 Features SfM2DFeatureUtilities::extractFeatures(const cv::Mat& image) {
-    static_assert(sizeof(cv::KeyPoint) == sizeof(sfmb200_keypoint), "cv::KeyPoint must be the 28-byte record of the ABI");
-    Features features;
-    if (image.empty()) return features;
+    if (image.empty()) return Features();
     const cv::Mat img = image.isContinuous() ? image : image.clone();
     const int nfeatures = 5000;                                                    // ORB::create(5000), :39
     int cap = nfeatures + 64, n = 0;
@@ -86,13 +80,7 @@ Features SfM2DFeatureUtilities::extractFeatures(const cv::Mat& image) {
         if (n <= cap) break;
         cap = n;                                                                   // ties at a selection threshold: OpenCV returns them all
     }
-    features.keyPoints.resize(n);
-    if (n) std::memcpy((void*)features.keyPoints.data(), kp.data(), sizeof(sfmb200_keypoint) * (size_t)n);
-    features.descriptors = cv::Mat(n, 32, kType8U);
-    if (n) std::memcpy(features.descriptors.ptr<uint8_t>(0), desc.data(), 32 * (size_t)n);
-    features.points.clear();                                                       // KeyPointsToPoints, SfMCommon.cpp:89-94
-    for (const auto& k : features.keyPoints) features.points.push_back(k.pt);
-    return features;
+    return featuresFromOrbRecords(kp.data(), desc.data(), n);                     // + KeyPointsToPoints, SfMCommon.cpp:89-94
 }
 #endif  // SFMB200_SHIM_KEEP_ORB
 

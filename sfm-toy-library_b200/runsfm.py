@@ -132,19 +132,31 @@ class SfM:
         return sfm
 
     @classmethod
-    def from_directory(cls, path, readImages: Callable = None, extractAllFeatures: Callable = None, *, downscale: float = 1.0, **kw):
+    def from_directory(cls, path, readImages: Callable = None, extractAllFeatures: Callable = None, *, downscale: float = 1.0,
+                       readImagesAndFeatures: Callable = None, **kw):
         """SfM::setImagesDirectory (SfM.cpp:97-139): the .jpg / .png files of `path` (extension compared case-insensitively), sorted
         by name, read by the injected stage (default cv2.imread per file; stages.readImages decodes them all on the device), then
         from_images.  With downscale != 1 (main.cpp's -s) every image is resized as at :127-129, byte-identical to cv::resize: an
         injected readImages is called as readImages(files, downscale=...) and resizes in the same call (stages.readImages does so on
         the device); after cv2.imread, stages.resizeImages resizes them all in one device call.  K then follows from the
-        downscaled size (SfM.cpp:70-72)."""
+        downscaled size (SfM.cpp:70-72).
+        readImagesAndFeatures, when given, replaces readImages + extractAllFeatures: it is called as readImagesAndFeatures(files,
+        downscale=...) (stages.readImagesAndFeatures decodes, resizes and extracts on the device in one call) and returns
+        (images, features); K still follows from image 0's size."""
         import os
         names = sorted(f for f in os.listdir(path) if os.path.splitext(f)[1].lower() in (".jpg", ".png"))
         if not names:
             raise ValueError(f"Unable to find valid files in images directory (\"{path}\").")
         files = [os.path.join(path, f) for f in names]
         t0 = time.perf_counter()
+        if readImagesAndFeatures is not None:
+            images, feats = readImagesAndFeatures(files, downscale=downscale)
+            dt = time.perf_counter() - t0
+            h, w = images[0].shape[:2]
+            sfm = cls(list(feats), (w, h), **kw)
+            sfm.seconds["read"] = dt; sfm.calls["read"] = len(files)
+            sfm.seconds["extract"] = 0.0; sfm.calls["extract"] = len(files)
+            return sfm
         if readImages is None:
             import cv2
             images = [cv2.imread(f) for f in files]

@@ -116,6 +116,19 @@ def extractAllFeatures(images: List[np.ndarray], ctx=None) -> List[Features]:
     return [_features_from(k, d) for k, d in ctx.orb_detect_and_compute(list(images), ORB_FEATURES)]
 
 
+def readImagesAndFeatures(files: List[str], downscale: float = 1.0, ctx=None):
+    """readImages followed by extractFeatures on every image, with the images staying on the device in between
+    (sfmb200_decode_jpeg_extract_orb): returns (images, features), the images as readImages returns them and per image the
+    Features extractFeatures gives for it.  The images may differ in size (portrait and landscape shots of one folder)."""
+    ctx = ctx or default_context()
+    blobs = []
+    for f in files:
+        with open(f, "rb") as fh:
+            blobs.append(fh.read())
+    images, feats = ctx.decode_jpeg_orb(blobs, _reference_factor(downscale), ORB_FEATURES)
+    return images, [_features_from(k, d) for k, d in feats]
+
+
 def matchFeatures(featuresLeft: Features, featuresRight: Features, ctx=None) -> np.ndarray:
     """SfM2DFeatureUtilities::matchFeatures (SfM2DFeatureUtilities.cpp:53-71)."""
     ctx = ctx or default_context()
