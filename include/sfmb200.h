@@ -556,6 +556,54 @@ int sfmb200_decode_jpeg_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data
                                     int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
                                     uint8_t* const* out_bgr /* NULL: images not downloaded */, const size_t* out_stride);
 
+/* ---- f-3: PNG and JPEG files, decoded (and downscaled, and ORB-extracted) in one call ----------------------------- */
+/*
+ * setImagesDirectory collects .jpg and .png files (SfM.cpp:110) and imread reads both.  These calls take any mix of the two formats.
+ * PNG output is byte-identical to cv::imread(file, IMREAD_COLOR) with OpenCV 4.13 and libpng 1.6: B,G,R; grey at 1/2/4/8/16 bits,
+ * RGB, palette, grey+alpha and RGBA at every legal depth; sub-byte grey scaled to 8 bits (a 1-bit 1 gives 255); 16-bit samples keep
+ * their high byte (0x12ff -> 0x12); alpha dropped without compositing; tRNS, gAMA, sRGB, iCCP, sBIT, cHRM ignored; a palette index
+ * past the end of PLTE gives (0,0,0); Adam7 interlacing; the EXIF orientation of an eXIf chunk (before or after IDAT) applied --
+ * orientations 5-8 swap width and height.  A CRC error in an ancillary chunk drops that chunk (a bad eXIf does not rotate).
+ * SFMB200_ERR_INVALID: a CRC error in a critical chunk, no IEND, a truncated file, an invalid zlib header or deflate stream (BTYPE 3,
+ * a stored LEN / NLEN mismatch, an over-subscribed or wrongly incomplete code, a bad code-length repeat, a distance before the start),
+ * too little image data, a filter type above 4, an Adler-32 mismatch, or any other file cv::imread refuses.  Extra compressed data
+ * after the image, or bytes after the zlib stream, still decode.  SFMB200_ERR_UNSUPPORTED: an animated PNG (acTL chunk), more than
+ * 65535 files, more than 512 MB of IDAT data in one call, an image with more than 2^31 - 1 bytes of filtered data.  Unlike libpng,
+ * nothing is padded or repaired; sfmb200_last_error names the image by its index in the caller's list.
+ *
+ * The deflate streams decode on the device.  Every bit offset is tested for the start of a dynamic-Huffman block whose header zlib
+ * would accept, and every such candidate is decoded to its end-of-block in parallel.  One thread per image then walks the true block
+ * sequence from the first block, taking a probed candidate wherever one starts at its position and decoding stored, fixed-Huffman
+ * and unprobed blocks itself (a Z_FIXED stream therefore decodes serially: correct, but slower than cv::imread).  Every block is then
+ * decoded again in parallel into one word per output byte, and back-references across blocks are resolved by pointer jumping.
+ * Unfiltering, Adam7, palette and colour conversion, orientation and the downscale follow on the device.  PNG images run in
+ * consecutive groups whose transient device memory (IDAT data, candidates, 5 bytes per filtered byte, block records) stays within
+ * SFMB200_PNG_GROUP_BYTES (an image larger than that runs alone); each group makes one upload, one download and one host
+ * synchronisation.
+ *
+ * sfmb200_image_info: host only (no context, no GPU): *format = SFMB200_FORMAT_JPEG or _PNG by signature, the output size after
+ * orientation, or the status a decode would return (SFMB200_ERR_INVALID for a file that is neither JPEG nor PNG).
+ * sfmb200_decode_images: as sfmb200_decode_jpeg_batch_scaled for any mix of JPEG and PNG files (scale == 1: no downscale).  Every file
+ * of both formats is parsed before anything launches.  An all-JPEG list gives exactly the JPEG calls' bytes and statistics.  A mixed
+ * list runs one JPEG decode (sfmb200_jpeg_last_stats describes it) and one PNG decode.
+ * sfmb200_decode_images_extract_orb: sfmb200_decode_jpeg_extract_orb for any mix of JPEG and PNG files: one ORB pass over all images,
+ * in the caller's order, with the same output contract.
+ * sfmb200_png_last_stats: the PNG part of the last call, SFMB200_PNG_STATS entries: [0] deflate blocks, [1] blocks the chain took
+ * from a probed candidate, [2] blocks the chain decoded itself, [3] candidates probed, [4] resolution rounds run until one changed
+ * nothing, summed over groups, [5] bytes uploaded, [6] bytes downloaded, [7] groups, [8] stored blocks, [9] fixed-Huffman blocks.
+ */
+#define SFMB200_FORMAT_JPEG 1
+#define SFMB200_FORMAT_PNG 2
+#define SFMB200_PNG_STATS 10
+#define SFMB200_PNG_GROUP_BYTES (1ull << 30)
+int sfmb200_image_info(const uint8_t* data, size_t size, int* format, int* width, int* height);
+int sfmb200_decode_images(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
+                          const size_t* out_stride);
+int sfmb200_decode_images_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, int nfeatures,
+                                      int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
+                                      uint8_t* const* out_bgr /* NULL: images not downloaded */, const size_t* out_stride);
+int sfmb200_png_last_stats(const sfmb200_ctx* ctx, int64_t* stats /* [SFMB200_PNG_STATS] */);
+
 /* ---- multi-GPU plumbing (NCCL, one process per GPU) ------------------------------------------------------ */
 #define SFMB200_UNIQUE_ID_BYTES 128
 int sfmb200_comm_unique_id(uint8_t* id /* [SFMB200_UNIQUE_ID_BYTES] */);       /* rank 0, then broadcast by the host */

@@ -526,6 +526,63 @@ class Context:
             feats.append((k, desc[i, :cnt[i]].copy()))
         return outs, feats
 
+    def _image_outputs(self, files, scale):
+        outs = []
+        for f in files:
+            rc, _, w, h = image_info(f)
+            if rc == 0 and scale != 1.0:
+                w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
+            outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
+        return outs
+
+    def decode_images(self, files, scale=1.0):
+        """sfmb200_decode_images: decode_jpeg for any mix of JPEG and PNG files (bytes), each byte-identical to
+        cv2.imdecode(buf, IMREAD_COLOR), then resized as cv2.resize(img, None, fx=scale, fy=scale) when scale != 1."""
+        files = [bytes(f) for f in files]
+        n = len(files)
+        scale = float(scale)
+        if n == 0:
+            return []
+        outs = self._image_outputs(files, scale)
+        data = (C.c_char_p * n)(*files)
+        sizes = (C.c_size_t * n)(*[len(f) for f in files])
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        self._check(lib().sfmb200_decode_images(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
+        return outs
+
+    def decode_images_orb(self, files, scale=1.0, nfeatures=5000, capacity=None, images=True):
+        """sfmb200_decode_images_extract_orb: decode_jpeg_orb for any mix of JPEG and PNG files; same returns and capacity retry."""
+        files = [bytes(f) for f in files]
+        n = len(files)
+        scale = float(scale)
+        if n == 0:
+            return ([] if images else None), []
+        outs = self._image_outputs(files, scale) if images else None
+        data = (C.c_char_p * n)(*files)
+        sizes = (C.c_size_t * n)(*[len(f) for f in files])
+        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs]) if images else None
+        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
+        while True:
+            kp = np.zeros((n, max(cap, 1), 7), np.float32); desc = np.zeros((n, max(cap, 1), 32), np.uint8); cnt = np.zeros(n, np.int32)
+            self._check(lib().sfmb200_decode_images_extract_orb(self._h, data, sizes, n, C.c_double(scale), int(nfeatures), cap,
+                                                                _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32), ptrs, None))
+            if cnt.max(initial=0) <= cap:
+                break
+            cap = int(cnt.max())                      # ties at a selection threshold: more key points than asked for
+        feats = []
+        for i in range(n):
+            k = kp[i, :cnt[i]].copy()
+            k[:, 5:7] = k[:, 5:7].view(np.int32).astype(np.float32)      # octave, class_id are int32 in the record
+            feats.append((k, desc[i, :cnt[i]].copy()))
+        return outs, feats
+
+    def png_last_stats(self):
+        """PNG counters of the last decode_images[_orb] call (sfmb200_png_last_stats)."""
+        s = np.zeros(PNG_STATS, np.int64)
+        self._check(lib().sfmb200_png_last_stats(self._h, _p(s, C.c_int64)))
+        return dict(zip(("blocks", "speculative_blocks", "chain_blocks", "candidates", "rounds", "upload_bytes", "download_bytes", "groups",
+                         "stored_blocks", "fixed_blocks"), s.tolist()))
+
     def resize_images(self, images, scale):
         """sfmb200_resize_batch: `images` is a list of uint8 [h, w, 3] B,G,R arrays (any sizes, strided rows allowed); returns them
         resized by `scale`, byte-identical to cv2.resize(img, None, fx=scale, fy=scale) (INTER_LINEAR), in one call.  A refused scale
@@ -599,6 +656,21 @@ def jpeg_info(data):
     w = C.c_int(0); h = C.c_int(0); c = C.c_int(0)
     rc = lib().sfmb200_jpeg_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(c))
     return int(rc), w.value, h.value, c.value
+
+
+FORMAT_JPEG, FORMAT_PNG = 1, 2
+PNG_STATS = 10
+PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
+
+
+def image_info(data):
+    """sfmb200_image_info: (status, format, width, height) of a JPEG or PNG file given as bytes, without a context or a GPU.  format is
+    FORMAT_JPEG or FORMAT_PNG; width and height are the decoded image's (after EXIF orientation); status 0 = decodable, 1 = invalid
+    (also for a file that is neither JPEG nor PNG), 5 = unsupported."""
+    data = bytes(data)
+    f = C.c_int(0); w = C.c_int(0); h = C.c_int(0)
+    rc = lib().sfmb200_image_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(f), C.byref(w), C.byref(h))
+    return int(rc), f.value, w.value, h.value
 
 
 def resize_size(width, height, scale):

@@ -130,6 +130,9 @@ struct sfmb200_ctx {
     DevBuf jpeg_dev;                    // JPEG decoding (jpeg.cu): tables, entropy data, coefficients, planes, images of the last batch
     PinBuf jpeg_pin_up, jpeg_pin_down;  // its one upload and its one download
     int64_t jpeg_stats[7] = {0, 0, 0, 0, 0, 0, 0};   // sfmb200_jpeg_last_stats of the last batch
+    DevBuf png_dev;                     // PNG decoding (png.cu): the images of the last call, then one group's IDAT data and work arrays
+    PinBuf png_pin_up, png_pin_down;    // a group's one upload and its one download
+    int64_t png_stats[SFMB200_PNG_STATS] = {};       // sfmb200_png_last_stats of the last call
     DevBuf rz_dev;                      // image downscale (resize.cu): descriptors, taps, source and resized images of the last batch
     PinBuf rz_pin_up, rz_pin_down;      // its one upload and its one download
 };

@@ -94,6 +94,7 @@ void sfmb200_destroy(sfmb200_ctx* ctx) {
     ctx->pose_trace.release();
     ctx->hg_trace.release();
     ctx->jpeg_dev.release(); ctx->jpeg_pin_up.release(); ctx->jpeg_pin_down.release();
+    ctx->png_dev.release(); ctx->png_pin_up.release(); ctx->png_pin_down.release();
     ctx->rz_dev.release(); ctx->rz_pin_up.release(); ctx->rz_pin_down.release();
     cudaStreamDestroy(ctx->stream);
     delete ctx;

@@ -357,8 +357,9 @@ struct JdResident { std::vector<const uint8_t*> ptr; std::vector<int> w, h; };
 // also stay where they are for the caller, each refused unless ORB can take it (8 <= width, height; at most 2^28 pixels), and out_bgr
 // may be null: then only the error words and the statistics come back.
 static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
-                     const size_t* out_stride, JdResident* res = nullptr) {
+                     const size_t* out_stride, JdResident* res = nullptr, const int* name = nullptr) {
     if (!ctx) return SFMB200_ERR_INVALID;
+    auto nm = [&](int i) { return name ? name[i] : i; };    // the image's index in the caller's list
     if (n < 0 || (n > 0 && (!data || !size || (!out_bgr && !res)))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: bad arguments");
     if (n > 65535) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: at most 65535 images per call");
     if (!std::isfinite(scale) || scale <= 0)
@@ -376,8 +377,8 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     std::vector<std::string> whys(n);
     pool.parallel_for(n, [&](int i) { rcs[i] = jp_parse(data[i], size[i], JD_CHUNK, ims[i], whys[i]); });
     for (int i = 0; i < n; ++i) {
-        if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", i, whys[i].c_str());
-        if (out_bgr && !out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", i);
+        if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", nm(i), whys[i].c_str());
+        if (out_bgr && !out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", nm(i));
     }
     // ---- the downscale: output sizes and taps of every image
     std::vector<RzImg> rz(scaled ? n : 0);
@@ -386,16 +387,16 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
         for (int i = 0; i < n; ++i) { memset(&rz[i], 0, sizeof(RzImg)); rz[i].sw = ims[i].OW; rz[i].sh = ims[i].OH; }
         int bad = 0;
         if (!rz_plan(scale, rz.data(), n, taps, &bad))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", bad, scale, ims[bad].OW, ims[bad].OH);
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", nm(bad), scale, ims[bad].OW, ims[bad].OH);
     }
     for (int i = 0; i < n; ++i) {
         const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
         if (out_bgr && out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", i, out_stride[i], ow * 3);
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", nm(i), out_stride[i], ow * 3);
         if (res && (ow < 8 || oh < 8))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: a %dx%d image is below ORB's minimum of 8 pixels per side", i, ow, oh);
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: a %dx%d image is below ORB's minimum of 8 pixels per side", nm(i), ow, oh);
         if (res && (int64_t)ow * oh > ((int64_t)1 << 28))
-            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image %d: a %dx%d image is too large for ORB (limit 2^28 pixels)", i, ow, oh);
+            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image %d: a %dx%d image is too large for ORB (limit 2^28 pixels)", nm(i), ow, oh);
     }
 
     // ---- layout
@@ -447,7 +448,7 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
             s.nsub = std::max<int>(1, (int)((s.b1 - s.b0 + JD_SUB - 1) / JD_SUB)); s.first_sub = 0;
             segs.push_back(s);
         }
-        if (ubytes != u) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: inconsistent scan walk", i);
+        if (ubytes != u) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: inconsistent scan walk", nm(i));
         if (in_bytes >= (1ull << 29)) return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "decode_jpeg_batch: more than 512 MB of entropy-coded data in one call");
     }
     int nsub = 0;
@@ -565,7 +566,7 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     const int* herr = (const int*)(hd + o_err);
     for (int i = 0; i < n; ++i)
         if (herr[i])
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: %s", i,
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: %s", nm(i),
                                 herr[i] & JD_ERR_DATA ? "corrupt entropy-coded data (no Huffman code, overrun or a run past coefficient 63)"
                                                       : "entropy-coded data ends before the last block");
     if (res) {
@@ -583,6 +584,16 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
         if (stride == row) memcpy(out_bgr[i], src, row * oh);
         else for (int y = 0; y < oh; ++y) memcpy(out_bgr[i] + y * stride, src + y * row, row);
     });
+    return SFMB200_OK;
+}
+
+// jd_decode for the mixed-format entry points (png.cu): messages name image i as name[i] (NULL: i), and with res_ptr the images stay
+// on the device as with `res`.
+int jd_decode_named(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, const int* name, int n, double scale, uint8_t* const* out_bgr,
+                    const size_t* out_stride, std::vector<const uint8_t*>* res_ptr, std::vector<int>* res_w, std::vector<int>* res_h) {
+    JdResident res;
+    if (int rc = jd_decode(ctx, data, size, n, scale, out_bgr, out_stride, res_ptr ? &res : nullptr, name)) return rc;
+    if (res_ptr) { *res_ptr = res.ptr; *res_w = res.w; *res_h = res.h; }
     return SFMB200_OK;
 }
 

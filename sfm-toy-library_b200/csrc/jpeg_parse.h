@@ -42,12 +42,10 @@ struct JpParser {
     int u16(size_t p) const { return (d[p] << 8) | d[p + 1]; }
 };
 
-// EXIF orientation the way cv::imdecode reads it (ExifReader): the first APP1 segment, 6 bytes skipped without looking at them, the
-// TIFF byte order ("II" little endian, anything else big endian), the 0x2A mark, IFD0, the first entry with tag 0x0112 and the
-// 16-bit value at +8 of the entry.  Entries are read until one would leave the segment.
-inline int jp_exif_orientation(const uint8_t* a, size_t len) {
-    if (len <= 6) return 1;
-    const uint8_t* t = a + 6; const size_t m = len - 6;
+// EXIF orientation the way cv::imdecode reads it (ExifReader) from the TIFF structure t [m bytes]: the byte order ("II" little endian,
+// anything else big endian), the 0x2A mark, IFD0, the first entry with tag 0x0112 and the 16-bit value at +8 of the entry.  Entries
+// are read until one would leave the structure.  The PNG decoder reads its eXIf chunk with it.
+inline int jp_tiff_orientation(const uint8_t* t, size_t m) {
     const bool le = m > 1 && t[0] == 'I' && t[1] == 'I';
     auto get16 = [&](size_t o, int& v) { if (o + 1 >= m) return false; v = le ? t[o] | (t[o + 1] << 8) : (t[o] << 8) | t[o + 1]; return true; };
     int mark = 0;
@@ -63,6 +61,12 @@ inline int jp_exif_orientation(const uint8_t* a, size_t len) {
         if (tag == 0x0112) return get16(o + 8, v) && v >= 1 && v <= 8 ? v : 1;
     }
     return 1;
+}
+
+// The same from a JPEG's first APP1 segment, whose 6 leading bytes are skipped without looking at them.
+inline int jp_exif_orientation(const uint8_t* a, size_t len) {
+    if (len <= 6) return 1;
+    return jp_tiff_orientation(a + 6, len - 6);
 }
 
 // Parses the file and walks its scan.  chunk = the unstuffing chunk size (bytes) seg_skip is counted in.  Returns JP_* with the

@@ -1,5 +1,5 @@
-// sfm_images.cpp -- sfmtoylib::readImages (sfm_images.h) over sfmb200_jpeg_info / sfmb200_decode_jpeg_batch, or with a downscale
-// sfmb200_resize_size / sfmb200_decode_jpeg_batch_scaled; sfmtoylib::readImagesAndFeatures over sfmb200_decode_jpeg_extract_orb.
+// sfm_images.cpp -- sfmtoylib::readImages (sfm_images.h) over sfmb200_image_info / sfmb200_resize_size / sfmb200_decode_images;
+// sfmtoylib::readImagesAndFeatures over sfmb200_decode_images_extract_orb.  Both take any mix of JPEG and PNG files.
 #include "sfm_images.h"
 #include "../../include/sfmb200.h"
 #include "sfm_features.h"
@@ -52,9 +52,9 @@ bool load(const std::vector<std::string>& filenames, double scale, float downsca
         if (!f) { std::cerr << "Unable to read image from file: " << filenames[i] << std::endl; return false; }
         b.files[i].assign(std::istreambuf_iterator<char>(f), std::istreambuf_iterator<char>());
         b.data[i] = b.files[i].data(); b.size[i] = b.files[i].size();
-        int w = 0, h = 0, c = 0;
-        if (sfmb200_jpeg_info(b.data[i], b.size[i], &w, &h, &c) != SFMB200_OK) {
-            std::cerr << "Unable to read image from file: " << filenames[i] << " (not a JPEG file the GPU decoder supports)" << std::endl;
+        int format = 0, w = 0, h = 0;
+        if (sfmb200_image_info(b.data[i], b.size[i], &format, &w, &h) != SFMB200_OK) {
+            std::cerr << "Unable to read image from file: " << filenames[i] << " (" << sfmb200_last_error(nullptr) << ")" << std::endl;
             return false;
         }
         if (scale != 1.0 && sfmb200_resize_size(w, h, scale, &w, &h) != SFMB200_OK) {
@@ -76,10 +76,8 @@ bool readImages(const std::vector<std::string>& filenames, std::vector<cv::Mat>&
     sfmb200_ctx* ctx = context();
     if (!ctx) return false;
     const int n = (int)b.files.size();
-    const int rc = scale == 1.0 ? sfmb200_decode_jpeg_batch(ctx, b.data.data(), b.size.data(), n, b.dst.data(), nullptr)
-                                : sfmb200_decode_jpeg_batch_scaled(ctx, b.data.data(), b.size.data(), n, scale, b.dst.data(), nullptr);
-    if (rc != SFMB200_OK) {
-        std::cerr << "sfmb200: decode_jpeg_batch: " << sfmb200_last_error(ctx) << std::endl;
+    if (sfmb200_decode_images(ctx, b.data.data(), b.size.data(), n, scale, b.dst.data(), nullptr) != SFMB200_OK) {
+        std::cerr << "sfmb200: decode_images: " << sfmb200_last_error(ctx) << std::endl;
         return false;
     }
     images.insert(images.end(), b.out.begin(), b.out.end());
@@ -100,9 +98,9 @@ bool readImagesAndFeatures(const std::vector<std::string>& filenames, std::vecto
     std::vector<int32_t> cnt(n);
     for (;;) {
         kp.resize((size_t)n * cap); desc.resize((size_t)n * cap * 32);
-        if (sfmb200_decode_jpeg_extract_orb(ctx, b.data.data(), b.size.data(), n, scale, nfeatures, cap, kp.data(), desc.data(), cnt.data(),
-                                            b.dst.data(), nullptr) != SFMB200_OK) {
-            std::cerr << "sfmb200: decode_jpeg_extract_orb: " << sfmb200_last_error(ctx) << std::endl;
+        if (sfmb200_decode_images_extract_orb(ctx, b.data.data(), b.size.data(), n, scale, nfeatures, cap, kp.data(), desc.data(), cnt.data(),
+                                              b.dst.data(), nullptr) != SFMB200_OK) {
+            std::cerr << "sfmb200: decode_images_extract_orb: " << sfmb200_last_error(ctx) << std::endl;
             return false;
         }
         const int most = n ? *std::max_element(cnt.begin(), cnt.end()) : 0;

@@ -69,17 +69,29 @@ def _reference_factor(downscale) -> float:
     return float(np.float32(downscale))
 
 
-def readImages(files: List[str], ctx=None, downscale: float = 1.0) -> List[np.ndarray]:
-    """The imread loop of SfM::setImagesDirectory (SfM.cpp:123-135) on the device: every file decoded in one
-    sfmb200_decode_jpeg_batch call, byte-identical to cv2.imread(file) (B,G,R, EXIF orientation applied).  With downscale != 1 the
-    loop's resize (:127-129) runs on the device in the same call (sfmb200_decode_jpeg_batch_scaled), byte-identical to
-    cv2.resize(cv2.imread(file), None, fx=s, fy=s) with s the factor as the reference's float.  Only JPEG files decode (there is
-    no host fallback): any other file raises capi.SfmB200Error naming it."""
-    ctx = ctx or default_context()
+def _read_files(files: List[str]) -> List[bytes]:
     blobs = []
     for f in files:
         with open(f, "rb") as fh:
             blobs.append(fh.read())
+    return blobs
+
+
+def _any_png(blobs: List[bytes]) -> bool:
+    return any(b[:8] == capi.PNG_SIGNATURE for b in blobs)
+
+
+def readImages(files: List[str], ctx=None, downscale: float = 1.0) -> List[np.ndarray]:
+    """The imread loop of SfM::setImagesDirectory (SfM.cpp:123-135) on the device: every file decoded in one call, byte-identical to
+    cv2.imread(file) (B,G,R, EXIF orientation applied).  The reference reads .jpg and .png files; a list with any PNG file goes to
+    sfmb200_decode_images (any mix of the two formats), an all-JPEG list to sfmb200_decode_jpeg_batch.  With downscale != 1 the
+    loop's resize (:127-129) runs on the device in the same call, byte-identical to cv2.resize(cv2.imread(file), None, fx=s, fy=s)
+    with s the factor as the reference's float.  There is no host fallback: a file that is neither JPEG nor PNG, or a corrupt or
+    unsupported one, raises capi.SfmB200Error naming it."""
+    ctx = ctx or default_context()
+    blobs = _read_files(files)
+    if _any_png(blobs):
+        return ctx.decode_images(blobs, _reference_factor(downscale))
     return ctx.decode_jpeg(blobs, _reference_factor(downscale))
 
 
@@ -118,14 +130,15 @@ def extractAllFeatures(images: List[np.ndarray], ctx=None) -> List[Features]:
 
 def readImagesAndFeatures(files: List[str], downscale: float = 1.0, ctx=None):
     """readImages followed by extractFeatures on every image, with the images staying on the device in between
-    (sfmb200_decode_jpeg_extract_orb): returns (images, features), the images as readImages returns them and per image the
-    Features extractFeatures gives for it.  The images may differ in size (portrait and landscape shots of one folder)."""
+    (sfmb200_decode_jpeg_extract_orb, or sfmb200_decode_images_extract_orb when any file is a PNG): returns (images, features), the
+    images as readImages returns them and per image the Features extractFeatures gives for it.  The images may differ in size
+    (portrait and landscape shots of one folder) and format."""
     ctx = ctx or default_context()
-    blobs = []
-    for f in files:
-        with open(f, "rb") as fh:
-            blobs.append(fh.read())
-    images, feats = ctx.decode_jpeg_orb(blobs, _reference_factor(downscale), ORB_FEATURES)
+    blobs = _read_files(files)
+    if _any_png(blobs):
+        images, feats = ctx.decode_images_orb(blobs, _reference_factor(downscale), ORB_FEATURES)
+    else:
+        images, feats = ctx.decode_jpeg_orb(blobs, _reference_factor(downscale), ORB_FEATURES)
     return images, [_features_from(k, d) for k, d in feats]
 
 
