@@ -584,8 +584,8 @@ int sfmb200_decode_jpeg_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data
  * sfmb200_image_info: host only (no context, no GPU): *format = SFMB200_FORMAT_JPEG or _PNG by signature, the output size after
  * orientation, or the status a decode would return (SFMB200_ERR_INVALID for a file that is neither JPEG nor PNG).
  * sfmb200_decode_images: as sfmb200_decode_jpeg_batch_scaled for any mix of JPEG and PNG files (scale == 1: no downscale).  Every file
- * of both formats is parsed before anything launches.  An all-JPEG list gives exactly the JPEG calls' bytes and statistics.  A mixed
- * list runs one JPEG decode (sfmb200_jpeg_last_stats describes it) and one PNG decode.
+ * of both formats is parsed and checked before anything launches.  An all-JPEG list gives exactly the JPEG calls' bytes and
+ * statistics.  A mixed list runs one JPEG decode (sfmb200_jpeg_last_stats describes it) and one PNG decode.
  * sfmb200_decode_images_extract_orb: sfmb200_decode_jpeg_extract_orb for any mix of JPEG and PNG files: one ORB pass over all images,
  * in the caller's order, with the same output contract.
  * sfmb200_png_last_stats: the PNG part of the last call, SFMB200_PNG_STATS entries: [0] deflate blocks, [1] blocks the chain took

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libsfmb200.so")
-SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "pose.cu", "homography.cu", "orb.cu", "jpeg.cu", "png.cu", "resize.cu"]
+SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "pose.cu", "homography.cu", "orb.cu", "decode.cu", "jpeg.cu", "png.cu", "resize.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
@@ -125,7 +125,7 @@ def build_host_pose(force=False):
 
 
 def build_images(force=False):
-    """sfmtoylib::readImages (host/sfm_images.cpp: the imread loop of setImagesDirectory over sfmb200_decode_jpeg_batch) + its driver."""
+    """sfmtoylib::readImages (host/sfm_images.cpp: the imread loop of setImagesDirectory over sfmb200_decode_images) + its driver."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_images")
     os.makedirs(os.path.dirname(out), exist_ok=True)
     deps = [os.path.join(hdir, f) for f in ("sfm_images.cpp", "sfm_images.h", "sfm_features.h", "test_images.cpp", "sfmtoylib_b200.h", "cv_min.h")] + [SO]
@@ -140,7 +140,7 @@ def build_images(force=False):
 
 
 def build_images_features(force=False):
-    """sfmtoylib::readImagesAndFeatures (host/sfm_images.cpp: decode, downscale and ORB in one sfmb200_decode_jpeg_extract_orb call) +
+    """sfmtoylib::readImagesAndFeatures (host/sfm_images.cpp: decode, downscale and ORB in one sfmb200_decode_images_extract_orb call) +
     its driver."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_images_features")
     os.makedirs(os.path.dirname(out), exist_ok=True)

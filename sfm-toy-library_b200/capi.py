@@ -414,12 +414,19 @@ class Context:
         if any(im.shape != imgs[0].shape for im in imgs):
             raise SfmB200Error("batched ORB extraction needs equally sized images")
         n = len(imgs)
-        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
         ptrs = (C.c_void_p * n)(*[im.ctypes.data for im in imgs])
+        out = self._orb_call(n, nfeatures, capacity, lambda cap, kp, desc, cnt: lib().sfmb200_orb_detect_and_compute_batch(
+            self._h, ptrs, n, int(w), int(h), int(ch), C.c_size_t(0), int(nfeatures), cap, kp, desc, cnt))
+        return out[0] if single else out
+
+    def _orb_call(self, n, nfeatures, capacity, call):
+        """The capacity retry and the record unpacking of every ORB call: call(cap, kp, desc, cnt) fills the key point records [n, cap],
+        descriptors [n, cap, 32] and counts [n]; a count above the capacity repeats the call with that count.  Returns per image
+        (key points [k, 7] float32, descriptors [k, 32] uint8)."""
+        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
         while True:
             kp = np.zeros((n, max(cap, 1), 7), np.float32); desc = np.zeros((n, max(cap, 1), 32), np.uint8); cnt = np.zeros(n, np.int32)
-            self._check(lib().sfmb200_orb_detect_and_compute_batch(self._h, ptrs, n, int(w), int(h), int(ch), C.c_size_t(0), int(nfeatures), cap,
-                                                                   _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32)))
+            self._check(call(cap, _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32)))
             if cnt.max(initial=0) <= cap:
                 break
             cap = int(cnt.max())                      # ties at a selection threshold: more key points than asked for
@@ -428,7 +435,7 @@ class Context:
             k = kp[i, :cnt[i]].copy()
             k[:, 5:7] = k[:, 5:7].view(np.int32).astype(np.float32)      # octave, class_id are int32 in the record
             out.append((k, desc[i, :cnt[i]].copy()))
-        return out[0] if single else out
+        return out
 
     def orb_prepare(self, images, nfeatures=5000, capacity=None):
         """Pre-marshalled form of orb_detect_and_compute for timing the C call itself: returns (call, kp, desc, cnt); call() runs
@@ -470,110 +477,48 @@ class Context:
         unsupported (status 5) or corrupt (status 1).  With scale != 1 (sfmb200_decode_jpeg_batch_scaled) every image is also
         downscaled on the device, byte-identical to cv2.resize(img, None, fx=scale, fy=scale), and only the resized images are
         downloaded."""
-        files = [bytes(f) for f in files]
-        n = len(files)
-        scale = float(scale)
-        if n == 0:
-            return []
-        outs = []
-        for f in files:
-            rc, w, h, _ = jpeg_info(f)
-            if rc == 0 and scale != 1.0:
-                w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
-            outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
-        data = (C.c_char_p * n)(*files)
-        sizes = (C.c_size_t * n)(*[len(f) for f in files])
-        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        if scale == 1.0:
-            self._check(lib().sfmb200_decode_jpeg_batch(self._h, data, sizes, n, ptrs, None))
-        else:
-            self._check(lib().sfmb200_decode_jpeg_batch_scaled(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
-        return outs
+        return self._decode(_decode_jpeg_batch if float(scale) == 1.0 else lib().sfmb200_decode_jpeg_batch_scaled, files, scale)
 
     def decode_jpeg_orb(self, files, scale=1.0, nfeatures=5000, capacity=None, images=True):
         """sfmb200_decode_jpeg_extract_orb: decode_jpeg(files, scale) and orb_detect_and_compute on every image in one call, with the
         images staying on the device in between; they may differ in size.  Returns (images or None, [(key points, descriptors), ...]):
         the images as decode_jpeg returns them when `images` is true (else they are not downloaded), and per image what
         orb_detect_and_compute returns for it.  A capacity below a key point count repeats the call with the count."""
-        files = [bytes(f) for f in files]
-        n = len(files)
-        scale = float(scale)
-        if n == 0:
-            return ([] if images else None), []
-        outs = None
-        if images:
-            outs = []
-            for f in files:
-                rc, w, h, _ = jpeg_info(f)
-                if rc == 0 and scale != 1.0:
-                    w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
-                outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))
-        data = (C.c_char_p * n)(*files)
-        sizes = (C.c_size_t * n)(*[len(f) for f in files])
-        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs]) if images else None
-        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
-        while True:
-            kp = np.zeros((n, max(cap, 1), 7), np.float32); desc = np.zeros((n, max(cap, 1), 32), np.uint8); cnt = np.zeros(n, np.int32)
-            self._check(lib().sfmb200_decode_jpeg_extract_orb(self._h, data, sizes, n, C.c_double(scale), int(nfeatures), cap,
-                                                              _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32), ptrs, None))
-            if cnt.max(initial=0) <= cap:
-                break
-            cap = int(cnt.max())                      # ties at a selection threshold: more key points than asked for
-        feats = []
-        for i in range(n):
-            k = kp[i, :cnt[i]].copy()
-            k[:, 5:7] = k[:, 5:7].view(np.int32).astype(np.float32)      # octave, class_id are int32 in the record
-            feats.append((k, desc[i, :cnt[i]].copy()))
-        return outs, feats
-
-    def _image_outputs(self, files, scale):
-        outs = []
-        for f in files:
-            rc, _, w, h = image_info(f)
-            if rc == 0 and scale != 1.0:
-                w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
-            outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
-        return outs
+        return self._decode(lib().sfmb200_decode_jpeg_extract_orb, files, scale, True, images, nfeatures, capacity)
 
     def decode_images(self, files, scale=1.0):
         """sfmb200_decode_images: decode_jpeg for any mix of JPEG and PNG files (bytes), each byte-identical to
         cv2.imdecode(buf, IMREAD_COLOR), then resized as cv2.resize(img, None, fx=scale, fy=scale) when scale != 1."""
-        files = [bytes(f) for f in files]
-        n = len(files)
-        scale = float(scale)
-        if n == 0:
-            return []
-        outs = self._image_outputs(files, scale)
-        data = (C.c_char_p * n)(*files)
-        sizes = (C.c_size_t * n)(*[len(f) for f in files])
-        ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        self._check(lib().sfmb200_decode_images(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
-        return outs
+        return self._decode(lib().sfmb200_decode_images, files, scale)
 
     def decode_images_orb(self, files, scale=1.0, nfeatures=5000, capacity=None, images=True):
         """sfmb200_decode_images_extract_orb: decode_jpeg_orb for any mix of JPEG and PNG files; same returns and capacity retry."""
+        return self._decode(lib().sfmb200_decode_images_extract_orb, files, scale, True, images, nfeatures, capacity)
+
+    def _decode(self, fn, files, scale, orb=False, images=True, nfeatures=5000, capacity=None):
+        """One call of the decode entry point fn over `files` (bytes).  Returns the images, or with `orb` (images or None, features),
+        as the public decode methods document."""
         files = [bytes(f) for f in files]
         n = len(files)
         scale = float(scale)
         if n == 0:
-            return ([] if images else None), []
-        outs = self._image_outputs(files, scale) if images else None
+            return (([] if images else None), []) if orb else []
+        outs = None
+        if images:
+            outs = []
+            for f in files:
+                rc, _, w, h = image_info(f)
+                if rc == 0 and scale != 1.0:
+                    w, h = resize_size(w, h, scale) or (1, 1)     # a refused scale fails the call below
+                outs.append(np.empty((h, w, 3) if rc == 0 else (1, 1, 3), np.uint8))    # a failing file fails the call below
         data = (C.c_char_p * n)(*files)
         sizes = (C.c_size_t * n)(*[len(f) for f in files])
         ptrs = (C.c_void_p * n)(*[o.ctypes.data for o in outs]) if images else None
-        cap = int(capacity) if capacity is not None else int(nfeatures) + 64
-        while True:
-            kp = np.zeros((n, max(cap, 1), 7), np.float32); desc = np.zeros((n, max(cap, 1), 32), np.uint8); cnt = np.zeros(n, np.int32)
-            self._check(lib().sfmb200_decode_images_extract_orb(self._h, data, sizes, n, C.c_double(scale), int(nfeatures), cap,
-                                                                _p(kp, C.c_float), _p(desc, C.c_uint8), _p(cnt, C.c_int32), ptrs, None))
-            if cnt.max(initial=0) <= cap:
-                break
-            cap = int(cnt.max())                      # ties at a selection threshold: more key points than asked for
-        feats = []
-        for i in range(n):
-            k = kp[i, :cnt[i]].copy()
-            k[:, 5:7] = k[:, 5:7].view(np.int32).astype(np.float32)      # octave, class_id are int32 in the record
-            feats.append((k, desc[i, :cnt[i]].copy()))
+        if not orb:
+            self._check(fn(self._h, data, sizes, n, C.c_double(scale), ptrs, None))
+            return outs
+        feats = self._orb_call(n, nfeatures, capacity, lambda cap, kp, desc, cnt: fn(self._h, data, sizes, n, C.c_double(scale), int(nfeatures),
+                                                                                   cap, kp, desc, cnt, ptrs, None))
         return outs, feats
 
     def png_last_stats(self):
@@ -656,6 +601,11 @@ def jpeg_info(data):
     w = C.c_int(0); h = C.c_int(0); c = C.c_int(0)
     rc = lib().sfmb200_jpeg_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(c))
     return int(rc), w.value, h.value, c.value
+
+
+def _decode_jpeg_batch(h, data, sizes, n, _scale, out_bgr, out_stride):
+    """sfmb200_decode_jpeg_batch with the arguments of the calls that take a scale."""
+    return lib().sfmb200_decode_jpeg_batch(h, data, sizes, n, out_bgr, out_stride)
 
 
 FORMAT_JPEG, FORMAT_PNG = 1, 2

@@ -44,16 +44,25 @@ struct PinBuf {
     void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
 
+// bytes rounded up to the 256-byte alignment of every buffer carved out of a DevBuf / PinBuf
+static inline size_t al256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
 // bump allocator over a DevBuf: carve() after a single reserve()
 struct Carver {
     char* base; size_t off = 0;
     explicit Carver(void* b) : base((char*)b) {}
     template <typename T> T* take(size_t n) {
-        off = (off + 255) & ~size_t(255);
+        off = al256(off);
         T* r = (T*)(base + off); off += n * sizeof(T); return r;
     }
-    static size_t pad(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+    static size_t pad(size_t bytes) { return al256(bytes); }
 };
+
+// h rows of `row` bytes from src (rows src_stride bytes apart) to dst (rows dst_stride bytes apart): one memcpy when both are packed.
+static inline void copy_rows(uint8_t* dst, size_t dst_stride, const uint8_t* src, size_t src_stride, size_t row, int h) {
+    if (dst_stride == row && src_stride == row) memcpy(dst, src, row * h);
+    else for (int y = 0; y < h; ++y) memcpy(dst + y * dst_stride, src + y * src_stride, row);
+}
 
 struct CommState;   // comm.cu
 
@@ -139,6 +148,12 @@ struct sfmb200_ctx {
 
 int sfmb200_fail(sfmb200_ctx* ctx, int code, const char* fmt, ...);
 
+// the context's host threads, created on first use
+static inline HostPool& host_pool(sfmb200_ctx* ctx) {
+    if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
+    return *ctx->pool;
+}
+
 // Host-side input checks shared by several entry points (ctx.cu).  Each returns SFMB200_OK, or SFMB200_ERR_INVALID with the
 // message set through sfmb200_fail.
 // check_pair_batch: the image-pair batch layout of include/sfmb200.h (pts / img_off / pairs / match_q / match_t / match_off) with
@@ -186,3 +201,24 @@ struct RzImg; struct RzTap;
 bool rz_plan(double scale, RzImg* imgs, int n, std::vector<RzTap>& taps, int* bad);
 int rz_enqueue(sfmb200_ctx* ctx, double scale, const RzImg* imgs, int n, const RzImg* d_imgs, const RzTap* d_taps, const uint8_t* d_src,
                uint8_t* d_dst);
+
+// image decoding: decode.cu checks a call and parses its files, then the JPEG (jpeg.cu) and PNG (png.cu) backends run them.
+constexpr int JD_CHUNK = 4096;        // bytes per unstuffing CTA of jpeg.cu, the unit jp_parse counts dropped bytes in
+
+// A decode call that has passed every check: the caller's arrays, indexed by the caller's image numbers, and every image's output size
+// (after the downscale).  The backend of image i sets dev[i] to where the image stays on the device, packed B,G,R rows, until the next
+// decode of its format.  out_bgr NULL: the images are not downloaded.
+struct DecodeCall {
+    const uint8_t* const* data;
+    double scale;
+    uint8_t* const* out_bgr;
+    const size_t* out_stride;
+    std::vector<int> ow, oh;
+    std::vector<const uint8_t*> dev;
+    size_t stride(int i) const { return out_stride && out_stride[i] ? out_stride[i] : (size_t)ow[i] * 3; }
+};
+// The call's files idx[k], parsed into ims[k].  Each backend refuses only what its device layout cannot hold, before its first launch,
+// and what its kernels find.
+struct JpImage; struct PgImage;
+int jd_run(sfmb200_ctx* ctx, DecodeCall& call, const std::vector<int>& idx, const std::vector<JpImage>& ims);
+int pg_run(sfmb200_ctx* ctx, DecodeCall& call, const std::vector<int>& idx, const std::vector<PgImage>& ims);

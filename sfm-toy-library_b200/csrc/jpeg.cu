@@ -1,7 +1,7 @@
-// jpeg.cu -- JPEG decoding of a batch of files on the device, byte-identical to cv::imread(IMREAD_COLOR) (include/sfmb200.h).
+// jpeg.cu -- the JPEG backend of the decode entry points (decode.cu checks a call and parses its files with jpeg_parse.h): JPEG files
+// decoded on the device, byte-identical to cv::imread(IMREAD_COLOR) (include/sfmb200.h).
 //
-// The host parses the markers (jpeg_parse.h) and packs the tables, the layout and the entropy-coded bytes of every image into one
-// pinned buffer: one upload.  On the device:
+// The host packs the tables, the layout and the entropy-coded bytes of every image into one pinned buffer: one upload.  On the device:
 //   jd_unstuff        removes the FF00 stuffing and the RSTn markers, one 4 KB chunk per CTA (block prefix sum of kept bytes)
 //   jd_sync0          every subsequence of JD_SUB bits decoded from a guessed state (block 0 of the MCU, DC)
 //   jd_sync_round     up to JD_ROUNDS rounds: a subsequence whose predecessor's exit moved is decoded again from that exit
@@ -11,7 +11,7 @@
 //   jd_dc_sum + scan + jd_dc_apply   DC prediction: per-component prefix sums over MCUs, reset at every restart segment
 //   jd_idct           dequantisation and jpeg_idct_islow, 8 threads per block, into uint8 component planes
 //   jd_color          upsampling, YCbCr -> B,G,R and the EXIF orientation, into the download area
-//   rz_*              (sfmb200_decode_jpeg_batch_scaled only) jd_color writes to device memory and the downscale of resize.cu
+//   rz_*              (scale != 1 only) jd_color writes to device memory and the downscale of resize.cu
 //                     writes the resized images into the download area instead
 // then one download (per-image error flags, statistics and the images) and one host synchronisation.
 #include "common.cuh"
@@ -20,7 +20,6 @@
 
 namespace {
 
-constexpr int JD_CHUNK = 4096;        // bytes per unstuffing CTA
 constexpr uint32_t JD_SUB = 1024;     // bits per subsequence
 constexpr int JD_ROUNDS = 6;          // parallel synchronisation rounds before the in-order sweep
 constexpr int JD_ERR_DATA = 1, JD_ERR_SHORT = 2;
@@ -344,59 +343,21 @@ __global__ void __launch_bounds__(256) jd_color(const JdImg* __restrict__ imgs, 
     o[0] = bgr[0]; o[1] = bgr[1]; o[2] = bgr[2];
 }
 
-size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
-
 }  // namespace
 
-// Images a decode leaves on the device (jd_decode with `res`): packed B,G,R rows of w[i] x h[i] pixels at ptr[i], inside ctx->jpeg_dev,
-// valid until the next decode.
-struct JdResident { std::vector<const uint8_t*> ptr; std::vector<int> w, h; };
-
-// Every decode entry point.  scale == 1: jd_color writes the images into the download area.  Otherwise jd_color writes them to device
-// memory, resize.cu's kernels downscale them into the download area, and only the resized images come back.  With `res` the images
-// also stay where they are for the caller, each refused unless ORB can take it (8 <= width, height; at most 2^28 pixels), and out_bgr
-// may be null: then only the error words and the statistics come back.
-static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
-                     const size_t* out_stride, JdResident* res = nullptr, const int* name = nullptr) {
-    if (!ctx) return SFMB200_ERR_INVALID;
-    auto nm = [&](int i) { return name ? name[i] : i; };    // the image's index in the caller's list
-    if (n < 0 || (n > 0 && (!data || !size || (!out_bgr && !res)))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: bad arguments");
-    if (n > 65535) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch: at most 65535 images per call");
-    if (!std::isfinite(scale) || scale <= 0)
-        return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_batch_scaled: scale %g is not a positive finite number", scale);
-    const bool scaled = scale != 1.0;
-    for (int i = 0; i < 7; ++i) ctx->jpeg_stats[i] = 0;
-    if (n == 0) return SFMB200_OK;
-    SFM_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
-    HostPool& pool = *ctx->pool;
-
-    // ---- parse every file (host threads)
-    std::vector<JpImage> ims(n);
-    std::vector<int> rcs(n, 0);
-    std::vector<std::string> whys(n);
-    pool.parallel_for(n, [&](int i) { rcs[i] = jp_parse(data[i], size[i], JD_CHUNK, ims[i], whys[i]); });
-    for (int i = 0; i < n; ++i) {
-        if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", nm(i), whys[i].c_str());
-        if (out_bgr && !out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", nm(i));
-    }
-    // ---- the downscale: output sizes and taps of every image
+// Decodes the JPEG files idx[i] of a checked call (decode.cu).  scale == 1: jd_color writes the images into the download area.
+// Otherwise jd_color writes them to device memory, resize.cu's kernels downscale them into the download area, and only the resized
+// images come back.  Without out_bgr only the error words and the statistics come back.
+int jd_run(sfmb200_ctx* ctx, DecodeCall& call, const std::vector<int>& idx, const std::vector<JpImage>& ims) {
+    const int n = (int)idx.size();
+    const bool scaled = call.scale != 1.0;
+    HostPool& pool = host_pool(ctx);
+    // ---- the downscale: taps of every image (decode.cu has checked the sizes)
     std::vector<RzImg> rz(scaled ? n : 0);
     std::vector<RzTap> taps;
     if (scaled) {
         for (int i = 0; i < n; ++i) { memset(&rz[i], 0, sizeof(RzImg)); rz[i].sw = ims[i].OW; rz[i].sh = ims[i].OH; }
-        int bad = 0;
-        if (!rz_plan(scale, rz.data(), n, taps, &bad))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", nm(bad), scale, ims[bad].OW, ims[bad].OH);
-    }
-    for (int i = 0; i < n; ++i) {
-        const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
-        if (out_bgr && out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", nm(i), out_stride[i], ow * 3);
-        if (res && (ow < 8 || oh < 8))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: a %dx%d image is below ORB's minimum of 8 pixels per side", nm(i), ow, oh);
-        if (res && (int64_t)ow * oh > ((int64_t)1 << 28))
-            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image %d: a %dx%d image is too large for ORB (limit 2^28 pixels)", nm(i), ow, oh);
+        rz_plan(call.scale, rz.data(), n, taps, nullptr);
     }
 
     // ---- layout
@@ -448,7 +409,7 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
             s.nsub = std::max<int>(1, (int)((s.b1 - s.b0 + JD_SUB - 1) / JD_SUB)); s.first_sub = 0;
             segs.push_back(s);
         }
-        if (ubytes != u) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: inconsistent scan walk", nm(i));
+        if (ubytes != u) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: inconsistent scan walk", idx[i]);
         if (in_bytes >= (1ull << 29)) return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "decode_jpeg_batch: more than 512 MB of entropy-coded data in one call");
     }
     int nsub = 0;
@@ -469,7 +430,7 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     pool.parallel_for(n, [&](int i) {
         memcpy(up + o_tabs + sizeof(JmHuff) * 8 * i, ims[i].tabs, sizeof(JmHuff) * 8);
         memcpy(up + o_qt + sizeof(int16_t) * 192 * i, ims[i].qt, sizeof(int16_t) * 192);
-        memcpy(up + o_in + in0[i], data[i] + ims[i].scan_off, ims[i].scan_len);
+        memcpy(up + o_in + in0[i], call.data[idx[i]] + ims[i].scan_off, ims[i].scan_len);
     });
     memcpy(up + o_img, img.data(), sizeof(JdImg) * n);
     memcpy(up + o_seg, segs.data(), sizeof(JdSeg) * nseg);
@@ -552,8 +513,8 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     jd_color<<<dim3((unsigned)ceil_div64(max_pix, 256), (unsigned)n), 256, 0, st>>>(d_img, d_planes, d_full);
     SFM_LAUNCH_CHECK(ctx);
     if (scaled)
-        if (int rc = rz_enqueue(ctx, scale, rz.data(), n, (const RzImg*)(dv + o_rzimg), (const RzTap*)(dv + o_rztap), d_full, d_out)) return rc;
-    const size_t got = out_bgr ? down_bytes : o_out;                 // images left on the device only: the error words and statistics
+        if (int rc = rz_enqueue(ctx, call.scale, rz.data(), n, (const RzImg*)(dv + o_rzimg), (const RzTap*)(dv + o_rztap), d_full, d_out)) return rc;
+    const size_t got = call.out_bgr ? down_bytes : o_out;            // images left on the device only: the error words and statistics
     SFM_CUDA(ctx, ctx->jpeg_pin_down.reserve(got));
     char* hd = (char*)ctx->jpeg_pin_down.p;
     SFM_CUDA(ctx, cudaMemcpyAsync(hd, down, got, cudaMemcpyDeviceToHost, st));
@@ -566,78 +527,25 @@ static int jd_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
     const int* herr = (const int*)(hd + o_err);
     for (int i = 0; i < n; ++i)
         if (herr[i])
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: %s", nm(i),
+            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: %s", idx[i],
                                 herr[i] & JD_ERR_DATA ? "corrupt entropy-coded data (no Huffman code, overrun or a run past coefficient 63)"
                                                       : "entropy-coded data ends before the last block");
-    if (res) {
-        res->ptr.resize(n); res->w.resize(n); res->h.resize(n);
-        for (int i = 0; i < n; ++i) {
-            res->ptr[i] = d_out + (scaled ? rz[i].dst0 : img[i].out0);
-            res->w[i] = scaled ? rz[i].dw : img[i].OW; res->h[i] = scaled ? rz[i].dh : img[i].OH;
-        }
-    }
-    if (!out_bgr) return SFMB200_OK;
+    for (int i = 0; i < n; ++i) call.dev[idx[i]] = d_out + (scaled ? rz[i].dst0 : img[i].out0);
+    if (!call.out_bgr) return SFMB200_OK;
     pool.parallel_for(n, [&](int i) {
-        const int ow = scaled ? rz[i].dw : img[i].OW, oh = scaled ? rz[i].dh : img[i].OH;
-        const size_t row = (size_t)ow * 3, stride = out_stride && out_stride[i] ? out_stride[i] : row;
-        const uint8_t* src = (const uint8_t*)(hd + o_out + (scaled ? rz[i].dst0 : img[i].out0));
-        if (stride == row) memcpy(out_bgr[i], src, row * oh);
-        else for (int y = 0; y < oh; ++y) memcpy(out_bgr[i] + y * stride, src + y * row, row);
+        const int j = idx[i];
+        const size_t row = (size_t)call.ow[j] * 3;
+        copy_rows(call.out_bgr[j], call.stride(j), (const uint8_t*)(hd + o_out + (scaled ? rz[i].dst0 : img[i].out0)), row, row, call.oh[j]);
     });
-    return SFMB200_OK;
-}
-
-// jd_decode for the mixed-format entry points (png.cu): messages name image i as name[i] (NULL: i), and with res_ptr the images stay
-// on the device as with `res`.
-int jd_decode_named(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, const int* name, int n, double scale, uint8_t* const* out_bgr,
-                    const size_t* out_stride, std::vector<const uint8_t*>* res_ptr, std::vector<int>* res_w, std::vector<int>* res_h) {
-    JdResident res;
-    if (int rc = jd_decode(ctx, data, size, n, scale, out_bgr, out_stride, res_ptr ? &res : nullptr, name)) return rc;
-    if (res_ptr) { *res_ptr = res.ptr; *res_w = res.w; *res_h = res.h; }
     return SFMB200_OK;
 }
 
 extern "C" {
 
-int sfmb200_jpeg_info(const uint8_t* data, size_t size, int* width, int* height, int* components) {
-    JpImage im; std::string why;
-    const int rc = jp_parse(data, size, JD_CHUNK, im, why);
-    if (rc) return rc;
-    if (width) *width = im.OW;
-    if (height) *height = im.OH;
-    if (components) *components = im.ncomp;
-    return SFMB200_OK;
-}
-
 int sfmb200_jpeg_last_stats(const sfmb200_ctx* ctx, int64_t* stats7) {
     if (!ctx || !stats7) return SFMB200_ERR_INVALID;
     for (int i = 0; i < 7; ++i) stats7[i] = ctx->jpeg_stats[i];
     return SFMB200_OK;
-}
-
-int sfmb200_decode_jpeg_batch(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, uint8_t* const* out_bgr,
-                              const size_t* out_stride) {
-    return jd_decode(ctx, data, size, n, 1.0, out_bgr, out_stride);
-}
-
-int sfmb200_decode_jpeg_batch_scaled(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale,
-                                     uint8_t* const* out_bgr, const size_t* out_stride) {
-    return jd_decode(ctx, data, size, n, scale, out_bgr, out_stride);
-}
-
-int sfmb200_decode_jpeg_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, int nfeatures,
-                                    int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
-                                    uint8_t* const* out_bgr, const size_t* out_stride) {
-    if (!ctx) return SFMB200_ERR_INVALID;
-    if (n < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_extract_orb: n < 0");
-    if (n == 0) return SFMB200_OK;
-    if (!keypoints || !descriptors || !n_keypoints || max_keypoints < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_jpeg_extract_orb: null buffer");
-    if (nfeatures < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "nfeatures < 0");
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    // The decode reads back its error words (with the images, if asked for) and fails on a bad file before ORB launches anything.
-    JdResident res;
-    if (int rc = jd_decode(ctx, data, size, n, scale, out_bgr, out_stride, &res)) return rc;
-    return orb_extract_device(ctx, res.ptr.data(), res.w.data(), res.h.data(), n, nfeatures, max_keypoints, keypoints, descriptors, n_keypoints);
 }
 
 }  // extern "C"

@@ -512,7 +512,7 @@ int orb_input_host(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, const O
     cudaStream_t up = ctx->orb_up;
     SFM_CUDA(ctx, cudaEventRecord(ctx->orb_ev[0], ctx->stream));         // the previous group's kernels have read the buffers the uploads overwrite
     SFM_CUDA(ctx, cudaStreamWaitEvent(up, ctx->orb_ev[0], 0));
-    ctx->pool->parallel_for(nb * PIECES, [&](int t) {
+    host_pool(ctx).parallel_for(nb * PIECES, [&](int t) {
         cudaSetDevice(dev);
         const int s = t / PIECES, c = t % PIECES;
         const OrbLayout& L = G.L[s];
@@ -541,7 +541,7 @@ int orb_input_host(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, const O
 int orb_finish(sfmb200_ctx* ctx, const OrbGroup& G, const OrbDev& D, int cap, KeyPointOut* kp_out, uint8_t* desc_out, int32_t* n_out,
                std::vector<std::vector<Rec>>& task, double t0) {
     cudaStream_t st = ctx->stream;
-    HostPool& pool = *ctx->pool;
+    HostPool& pool = host_pool(ctx);
     double* tm = ctx->orb_ms;
     const int nb = G.nb, i0 = G.i0;
     int max_rows = 0;
@@ -697,7 +697,6 @@ int orb_run(sfmb200_ctx* ctx, const OrbInput& in, int n_images, const int* ws, c
         SFM_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->orb_up, cudaStreamNonBlocking));
         for (auto& ev : ctx->orb_ev) SFM_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     }
-    if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
     double* tm = ctx->orb_ms;
     for (int i = 0; i < 8; i++) tm[i] = 0.0;
     SFM_CUDA(ctx, ctx->orb_dev.reserve(dev_need + 4096));

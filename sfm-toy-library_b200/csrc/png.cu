@@ -1,8 +1,7 @@
-// png.cu -- PNG decoding of a batch of files on the device, byte-identical to cv::imread(IMREAD_COLOR) (include/sfmb200.h), and the
-// entry points that decode any mix of JPEG and PNG files.
+// png.cu -- the PNG backend of the decode entry points (decode.cu checks a call and parses its files with png_parse.h): PNG files
+// decoded on the device, byte-identical to cv::imread(IMREAD_COLOR) (include/sfmb200.h).
 //
-// The host parses the chunks (png_parse.h) and packs the IDAT payloads of a group of images into one pinned buffer: one upload.  On
-// the device, per group:
+// The host packs the IDAT payloads of a group of images into one pinned buffer: one upload.  On the device, per group:
 //   pg_scan       one thread per window of 512 bit offsets keeps the first 4 offsets where a dynamic-Huffman block header zlib accepts
 //                 could start (HLIT, HDIST, a complete code-length code, the lengths, the literal/length and distance codes)
 //   pg_probe      one thread per candidate decodes it to its end-of-block: end bit and output bytes, or not a block
@@ -60,8 +59,6 @@ __device__ __forceinline__ int pg_image_of(long long k, int n, F first) {
     while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (first(mid) <= k) lo = mid; else hi = mid - 1; }
     return lo;
 }
-
-size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 // ---------------------------------------------------------------------------------------------------------------- inflate
 struct ChainSink {                       // counts output bytes and refuses a distance before the start of the stream
@@ -339,49 +336,18 @@ const char* pg_err_text(int e) {
 
 }  // namespace
 
-// Images a decode leaves on the device: packed B,G,R rows of w[i] x h[i] pixels at ptr[i] (png.cu: inside ctx->png_dev, valid until the
-// next PNG decode).
-struct PgResident { std::vector<const uint8_t*> ptr; std::vector<int> w, h; };
-
-// Decodes the n PNG files data[i] (named in messages as image idx[i]).  Groups of consecutive images whose transient device memory
-// fits SFMB200_PNG_GROUP_BYTES run one after the other, each with one upload, one download and one host synchronisation; the images
-// themselves stay on the device for the whole call.  out_bgr / out_stride / res as in jd_decode (jpeg.cu).
-static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, const int* idx, int n, double scale,
-                     uint8_t* const* out_bgr, const size_t* out_stride, PgResident* resid) {
-    const bool scaled = scale != 1.0;
-    for (int k = 0; k < SFMB200_PNG_STATS; ++k) ctx->png_stats[k] = 0;
-    if (n == 0) return SFMB200_OK;
-    SFM_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
-    HostPool& pool = *ctx->pool;
-    std::vector<PgImage> ims(n);
-    std::vector<int> rcs(n, 0);
-    std::vector<std::string> whys(n);
-    pool.parallel_for(n, [&](int i) { rcs[i] = pg_parse(data[i], size[i], ims[i], whys[i]); });
+// Decodes the PNG files idx[i] of a checked call (decode.cu).  Groups of consecutive images whose transient device memory fits
+// SFMB200_PNG_GROUP_BYTES run one after the other, each with one upload, one download and one host synchronisation; the images
+// themselves stay on the device for the whole call.
+int pg_run(sfmb200_ctx* ctx, DecodeCall& call, const std::vector<int>& idx, const std::vector<PgImage>& ims) {
+    const int n = (int)idx.size();
+    const bool scaled = call.scale != 1.0;
+    HostPool& pool = host_pool(ctx);
     size_t zall = 0;
-    for (int i = 0; i < n; ++i) {
-        if (rcs[i]) return sfmb200_fail(ctx, rcs[i], "image %d: %s", idx[i], whys[i].c_str());
-        if (out_bgr && !out_bgr[i]) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: no output buffer", idx[i]);
-        zall += ims[i].zlen;
-    }
+    for (const PgImage& p : ims) zall += p.zlen;
     if (zall >= (1ull << 29)) return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "decode_images: more than 512 MB of PNG image data in one call");
-    std::vector<RzImg> rz(scaled ? n : 0);
-    if (scaled) {
-        std::vector<RzTap> taps;
-        for (int i = 0; i < n; ++i) { memset(&rz[i], 0, sizeof(RzImg)); rz[i].sw = ims[i].OW; rz[i].sh = ims[i].OH; }
-        int bad = 0;
-        if (!rz_plan(scale, rz.data(), n, taps, &bad))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: scale %g of a %dx%d image gives no image", idx[bad], scale, ims[bad].OW, ims[bad].OH);
-    }
-    for (int i = 0; i < n; ++i) {
-        const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
-        if (out_bgr && out_stride && out_stride[i] && out_stride[i] < (size_t)ow * 3)
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", idx[i], out_stride[i], ow * 3);
-        if (resid && (ow < 8 || oh < 8))
-            return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: a %dx%d image is below ORB's minimum of 8 pixels per side", idx[i], ow, oh);
-        if (resid && (int64_t)ow * oh > ((int64_t)1 << 28))
-            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "image %d: a %dx%d image is too large for ORB (limit 2^28 pixels)", idx[i], ow, oh);
-    }
+    auto ow = [&](int i) { return call.ow[idx[i]]; };
+    auto oh = [&](int i) { return call.oh[idx[i]]; };
 
     // ---- groups: consecutive images whose transient device memory fits the budget (an image alone always runs)
     auto blkcap = [&](int i) { return (long long)(ims[i].zlen * 8 / 10 + 2); };
@@ -406,8 +372,7 @@ static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
         grp_off[g] = a;
         a += al256(sizeof(PgRes) * (g0[g + 1] - g0[g]) + sizeof(int) * (PG_ROUNDS + 1));
         for (int i = g0[g]; i < g0[g + 1]; ++i) {
-            const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
-            img_off[i] = a; a += al256((size_t)ow * oh * 3);
+            img_off[i] = a; a += al256((size_t)ow(i) * oh(i) * 3);
         }
     }
     grp_off[ngroups] = a;
@@ -452,8 +417,7 @@ static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
         if (scaled) {
             grz.resize(m);
             for (int k = 0; k < m; ++k) { memset(&grz[k], 0, sizeof(RzImg)); grz[k].sw = img[k].OW; grz[k].sh = img[k].OH; }
-            int bad = 0;
-            if (!rz_plan(scale, grz.data(), m, taps, &bad)) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: bad scale", idx[a0 + bad]);
+            rz_plan(call.scale, grz.data(), m, taps, nullptr);
             for (int k = 0; k < m; ++k) {
                 grz[k].src0 = img[k].out0; grz[k].src_stride = (long long)img[k].OW * 3;
                 grz[k].dst0 = (long long)(img_off[a0 + k] - grp_off[g]); grz[k].dst_stride = (long long)grz[k].dw * 3;
@@ -471,7 +435,7 @@ static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
             memcpy(up + o_pal + 768ull * k, p.pal, 768);
             char* zd = up + o_z + img[k].z0;
             size_t o = 0;
-            for (auto& c : p.idat) { memcpy(zd + o, data[a0 + k] + c.first, c.second); o += c.second; }
+            for (auto& c : p.idat) { memcpy(zd + o, call.data[idx[a0 + k]] + c.first, c.second); o += c.second; }
             memset(zd + o, 0, al256(p.zlen + 16) - o);
         });
         // ---- device memory of the group
@@ -526,8 +490,8 @@ static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
         pg_color<<<dim3((unsigned)ceil_div64(max_pix, 256), (unsigned)m), 256, 0, st>>>(d_img, d_r, d_pal, d_res, d_f);
         SFM_LAUNCH_CHECK(ctx);
         if (scaled)
-            if (int rc = rz_enqueue(ctx, scale, grz.data(), m, (const RzImg*)(dv + o_rz), (const RzTap*)(dv + o_tap), d_f, d_out)) return rc;
-        const size_t got = out_bgr ? grp_off[g + 1] - grp_off[g] : res_bytes;
+            if (int rc = rz_enqueue(ctx, call.scale, grz.data(), m, (const RzImg*)(dv + o_rz), (const RzTap*)(dv + o_tap), d_f, d_out)) return rc;
+        const size_t got = call.out_bgr ? grp_off[g + 1] - grp_off[g] : res_bytes;
         SFM_CUDA(ctx, ctx->png_pin_down.reserve(got));
         char* hd = (char*)ctx->png_pin_down.p;
         SFM_CUDA(ctx, cudaMemcpyAsync(hd, down, got, cudaMemcpyDeviceToHost, st));
@@ -548,154 +512,25 @@ static int pg_decode(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t*
             blocks += hr[k].nblocks; chain += hr[k].chain; stored += hr[k].stored; fixed += hr[k].fixed; spec += hr[k].spec;
             probed += hr[k].probed;
         }
-        if (out_bgr)
+        if (call.out_bgr)
             pool.parallel_for(m, [&](int k) {
-                const int i = a0 + k;
-                const int ow = scaled ? rz[i].dw : ims[i].OW, oh = scaled ? rz[i].dh : ims[i].OH;
-                const size_t row = (size_t)ow * 3, stride = out_stride && out_stride[i] ? out_stride[i] : row;
-                const uint8_t* src = (const uint8_t*)(hd + (img_off[i] - grp_off[g]));
-                if (stride == row) memcpy(out_bgr[i], src, row * oh);
-                else for (int y = 0; y < oh; ++y) memcpy(out_bgr[i] + y * stride, src + y * row, row);
+                const int i = a0 + k, j = idx[i];
+                const size_t row = (size_t)ow(i) * 3;
+                copy_rows(call.out_bgr[j], call.stride(j), (const uint8_t*)(hd + (img_off[i] - grp_off[g])), row, row, oh(i));
             });
     }
     int64_t* s = ctx->png_stats;
     s[0] = blocks; s[1] = spec; s[2] = chain; s[3] = probed; s[4] = rounds; s[5] = up_total; s[6] = down_total; s[7] = ngroups; s[8] = stored; s[9] = fixed;
-    if (resid) {
-        resid->ptr.resize(n); resid->w.resize(n); resid->h.resize(n);
-        for (int i = 0; i < n; ++i) {
-            resid->ptr[i] = (const uint8_t*)(keep + img_off[i]);
-            resid->w[i] = scaled ? rz[i].dw : ims[i].OW; resid->h[i] = scaled ? rz[i].dh : ims[i].OH;
-        }
-    }
+    for (int i = 0; i < n; ++i) call.dev[idx[i]] = (const uint8_t*)(keep + img_off[i]);
     return SFMB200_OK;
 }
-
-// The JPEG decoder's entry (jpeg.cu)
-int jd_decode_named(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, const int* idx, int n, double scale, uint8_t* const* out_bgr,
-                    const size_t* out_stride, std::vector<const uint8_t*>* res_ptr, std::vector<int>* res_w, std::vector<int>* res_h);
-
-namespace {
-
-constexpr int FMT_NONE = 0;
-
-int image_format(const uint8_t* d, size_t n) {
-    if (pg_is_png(d, n)) return SFMB200_FORMAT_PNG;
-    if (d && n >= 2 && d[0] == 0xFF && d[1] == 0xD8) return SFMB200_FORMAT_JPEG;
-    return FMT_NONE;
-}
-
-// Any mix of JPEG and PNG files: every file parsed before anything launches, then one JPEG decode and one PNG decode, each into its own
-// arena, so that with `res` both sets of images are alive on the device together.
-int decode_mixed(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
-                 const size_t* out_stride, PgResident* res) {
-    if (n < 0 || (n > 0 && (!data || !size || (!out_bgr && !res)))) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_images: bad arguments");
-    if (n > 65535) return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "decode_images: at most 65535 images per call");
-    if (!std::isfinite(scale) || scale <= 0)
-        return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_images: scale %g is not a positive finite number", scale);
-    for (int k = 0; k < SFMB200_PNG_STATS; ++k) ctx->png_stats[k] = 0;
-    std::vector<int> jpg, png;
-    for (int i = 0; i < n; ++i) {
-        const int f = image_format(data[i], size[i]);
-        if (f == FMT_NONE) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: neither a JPEG nor a PNG file", i);
-        (f == SFMB200_FORMAT_PNG ? png : jpg).push_back(i);
-    }
-    auto pick = [&](const std::vector<int>& ix, auto* arr) {
-        std::vector<std::remove_const_t<std::remove_pointer_t<decltype(arr)>>> v;
-        if (arr) for (int i : ix) v.push_back(arr[i]);
-        return v;
-    };
-    if (png.empty()) {                                     // all JPEG: exactly the JPEG decode
-        std::vector<const uint8_t*> rp; std::vector<int> rw, rh;
-        if (int rc = jd_decode_named(ctx, data, size, nullptr, n, scale, out_bgr, out_stride, res ? &rp : nullptr, &rw, &rh)) return rc;
-        if (res) { res->ptr = rp; res->w = rw; res->h = rh; }
-        return SFMB200_OK;
-    }
-    const auto pd = pick(png, data); const auto ps = pick(png, size);
-    const auto po = pick(png, out_bgr); const auto pst = pick(png, out_stride);
-    // with JPEG files in the list: parse every PNG (and with it fail on a bad one) before the JPEG decode launches anything; the JPEG
-    // decode parses its files before its own first launch
-    if (!jpg.empty()) {
-        std::vector<std::string> why(png.size());
-        std::vector<int> rc(png.size());
-        if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
-        ctx->pool->parallel_for((int)png.size(), [&](int k) { PgImage im; rc[k] = pg_parse(pd[k], ps[k], im, why[k]); });
-        for (size_t k = 0; k < png.size(); ++k)
-            if (rc[k]) return sfmb200_fail(ctx, rc[k], "image %d: %s", png[k], why[k].c_str());
-    }
-    std::vector<const uint8_t*> jp; std::vector<int> jw, jh;
-    if (!jpg.empty()) {
-        const auto jd = pick(jpg, data); const auto js = pick(jpg, size);
-        const auto jo = pick(jpg, out_bgr); const auto jst = pick(jpg, out_stride);
-        if (int rc = jd_decode_named(ctx, jd.data(), js.data(), jpg.data(), (int)jpg.size(), scale, out_bgr ? jo.data() : nullptr,
-                                     out_stride ? jst.data() : nullptr, res ? &jp : nullptr, &jw, &jh))
-            return rc;
-    } else {
-        for (int k = 0; k < 7; ++k) ctx->jpeg_stats[k] = 0;
-    }
-    PgResident pr;
-    if (int rc = pg_decode(ctx, pd.data(), ps.data(), png.data(), (int)png.size(), scale, out_bgr ? po.data() : nullptr,
-                           out_stride ? pst.data() : nullptr, res ? &pr : nullptr))
-        return rc;
-    if (res) {
-        res->ptr.resize(n); res->w.resize(n); res->h.resize(n);
-        for (size_t k = 0; k < jpg.size(); ++k) { res->ptr[jpg[k]] = jp[k]; res->w[jpg[k]] = jw[k]; res->h[jpg[k]] = jh[k]; }
-        for (size_t k = 0; k < png.size(); ++k) { res->ptr[png[k]] = pr.ptr[k]; res->w[png[k]] = pr.w[k]; res->h[png[k]] = pr.h[k]; }
-    }
-    return SFMB200_OK;
-}
-
-}  // namespace
 
 extern "C" {
-
-int sfmb200_image_info(const uint8_t* data, size_t size, int* format, int* width, int* height) {
-    // a refusal leaves its reason in sfmb200_last_error(NULL)
-    const int f = image_format(data, size);
-    int w = 0, h = 0;
-    std::string why;
-    if (f == SFMB200_FORMAT_PNG) {
-        PgImage im;
-        if (int rc = pg_parse(data, size, im, why)) return sfmb200_fail(nullptr, rc, "%s", why.c_str());
-        w = im.OW; h = im.OH;
-    } else if (f == SFMB200_FORMAT_JPEG) {
-        JpImage im;
-        if (int rc = jp_parse(data, size, 4096, im, why)) return sfmb200_fail(nullptr, rc, "%s", why.c_str());
-        w = im.OW; h = im.OH;
-    } else {
-        sfmb200_fail(nullptr, SFMB200_ERR_INVALID, "neither a JPEG nor a PNG file");
-        return SFMB200_ERR_INVALID;
-    }
-    if (format) *format = f;
-    if (width) *width = w;
-    if (height) *height = h;
-    return SFMB200_OK;
-}
 
 int sfmb200_png_last_stats(const sfmb200_ctx* ctx, int64_t* stats) {
     if (!ctx || !stats) return SFMB200_ERR_INVALID;
     for (int k = 0; k < SFMB200_PNG_STATS; ++k) stats[k] = ctx->png_stats[k];
     return SFMB200_OK;
-}
-
-int sfmb200_decode_images(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, uint8_t* const* out_bgr,
-                          const size_t* out_stride) {
-    if (!ctx) return SFMB200_ERR_INVALID;
-    if (n > 0 && !out_bgr) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_images: no output buffers");
-    return decode_mixed(ctx, data, size, n, scale, out_bgr, out_stride, nullptr);
-}
-
-int sfmb200_decode_images_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* data, const size_t* size, int n, double scale, int nfeatures,
-                                      int max_keypoints, sfmb200_keypoint* keypoints, uint8_t* descriptors, int32_t* n_keypoints,
-                                      uint8_t* const* out_bgr, const size_t* out_stride) {
-    if (!ctx) return SFMB200_ERR_INVALID;
-    if (n < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_images_extract_orb: n < 0");
-    if (n == 0) return SFMB200_OK;
-    if (!keypoints || !descriptors || !n_keypoints || max_keypoints < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "decode_images_extract_orb: null buffer");
-    if (nfeatures < 0) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "nfeatures < 0");
-    std::lock_guard<std::mutex> lk(ctx->mu);
-    PgResident res;
-    if (int rc = decode_mixed(ctx, data, size, n, scale, out_bgr, out_stride, &res)) return rc;
-    return orb_extract_device(ctx, res.ptr.data(), res.w.data(), res.h.data(), n, nfeatures, max_keypoints, keypoints, descriptors, n_keypoints);
 }
 
 }  // extern "C"

@@ -5,8 +5,8 @@
 //   rz_linear   one CTA per RZ_TW x RZ_TH output tile: the horizontal pass of the two source rows of every output row of the tile into
 //               shared memory (int32), then the vertical pass, packed B,G,R out
 //   rz_area     1 / s == 2: one thread per output pixel, the 2x2 block average with its edge rule
-// The taps are built on the host (rz_plan) and ride in the call's one upload.  sfmb200_decode_jpeg_batch_scaled (jpeg.cu) runs the
-// same kernels on the images jd_color has just written.
+// The taps are built on the host (rz_plan) and ride in the call's one upload.  The scaled decodes (jpeg.cu, png.cu) run the same kernels
+// on the images they have just decoded.
 #include "common.cuh"
 #include "resize_math.cuh"
 
@@ -46,8 +46,6 @@ __global__ void __launch_bounds__(256) rz_area(const RzImg* __restrict__ imgs, c
     uint8_t* o = dst + im.dst0 + dy * im.dst_stride + 3 * dx;
     for (int c = 0; c < 3; ++c) o[c] = rz_area2(src + im.src0, im.src_stride, im.sw, im.sh, dx, dy, c);
 }
-
-size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 }  // namespace
 
@@ -113,14 +111,11 @@ int sfmb200_resize_batch(sfmb200_ctx* ctx, const uint8_t* const* src, const int*
         if (dst_stride && dst_stride[i] && dst_stride[i] < (size_t)img[i].dw * 3)
             return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "image %d: output stride %zu < %d", i, dst_stride[i], img[i].dw * 3);
     if (n == 0) return SFMB200_OK;
-    if (!ctx->pool) ctx->pool = new HostPool(HostPool::default_threads() - 1);
-    HostPool& pool = *ctx->pool;
+    HostPool& pool = host_pool(ctx);
     auto srow = [&](int i) { return src_stride && src_stride[i] ? src_stride[i] : (size_t)w[i] * 3; };
     auto drow = [&](int i) { return dst_stride && dst_stride[i] ? dst_stride[i] : (size_t)img[i].dw * 3; };
     if (scale == 1.0) {                 // SfM::setImagesDirectory does not call cv::resize for a factor of 1: the input bytes
-        pool.parallel_for(n, [&](int i) {
-            for (int y = 0; y < h[i]; ++y) memcpy(dst[i] + y * drow(i), src[i] + y * srow(i), (size_t)w[i] * 3);
-        });
+        pool.parallel_for(n, [&](int i) { copy_rows(dst[i], drow(i), src[i], srow(i), (size_t)w[i] * 3, h[i]); });
         return SFMB200_OK;
     }
     SFM_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -141,10 +136,8 @@ int sfmb200_resize_batch(sfmb200_ctx* ctx, const uint8_t* const* src, const int*
     memcpy(up + o_img, img.data(), sizeof(RzImg) * n);
     memcpy(up + o_tap, taps.data(), sizeof(RzTap) * taps.size());
     pool.parallel_for(n, [&](int i) {
-        uint8_t* p = (uint8_t*)up + o_src + img[i].src0;
         const size_t row = (size_t)img[i].src_stride;
-        if (srow(i) == row) memcpy(p, src[i], row * img[i].sh);
-        else for (int y = 0; y < img[i].sh; ++y) memcpy(p + y * row, src[i] + y * srow(i), row);
+        copy_rows((uint8_t*)up + o_src + img[i].src0, row, src[i], srow(i), row, img[i].sh);
     });
     char* dv = (char*)ctx->rz_dev.p;
     cudaStream_t st = ctx->stream;
@@ -157,9 +150,7 @@ int sfmb200_resize_batch(sfmb200_ctx* ctx, const uint8_t* const* src, const int*
     SFM_CUDA(ctx, cudaStreamSynchronize(st));
     pool.parallel_for(n, [&](int i) {
         const size_t row = (size_t)img[i].dst_stride;
-        const uint8_t* p = (const uint8_t*)hd + img[i].dst0;
-        if (drow(i) == row) memcpy(dst[i], p, row * img[i].dh);
-        else for (int y = 0; y < img[i].dh; ++y) memcpy(dst[i] + y * drow(i), p + y * row, row);
+        copy_rows(dst[i], drow(i), (const uint8_t*)hd + img[i].dst0, row, row, img[i].dh);
     });
     return SFMB200_OK;
 }
