@@ -274,13 +274,23 @@ int sfmb200_ransac_score(sfmb200_ctx* ctx, int model, const float* a, const floa
  * findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118):
  *     E = findEssentialMat(left, right, focal, pp, RANSAC, 0.999, 1.0, mask);  recoverPose(E, left, right, R, t, focal, pp, mask);
  * in one call.  Points are normalised x = ((double)px - cx) / focal with focal = K[0], (cx, cy) = (K[2], K[5]); the threshold
- * becomes threshold_px / focal.  max_iters samples of 5 distinct correspondences are drawn from a counter-based generator
- * (splitmix64 keyed by seed, sample and draw; a repeated index is redrawn), every sample is solved by the five-point
- * solver (up to 10 E), every solution is scored with the Sampson error and inlier rule of sfmb200_ransac_score, and
- * OpenCV's sequential loop (RANSACPointSetRegistrator::run) is replayed over the counts in sample order: a solution
- * replaces the best one only if its count exceeds max(best count, 4), every improvement recomputes the sample budget with
- * RANSACUpdateNumIters(confidence, outlier ratio, 5, budget), and the loop stops at the budget.  The result is what that
- * loop returns on this sample sequence; cv:: draws its samples from its own RNG, so it agrees with cv:: only statistically.
+ * becomes threshold_px / focal.  max_iters samples of 5 distinct correspondences are drawn by the sampler the options name,
+ * every sample is solved by the five-point solver (up to 10 E, real roots in ascending order), every solution is scored with the
+ * Sampson error and inlier rule of sfmb200_ransac_score, and OpenCV's sequential loop (RANSACPointSetRegistrator::run) is replayed
+ * over the counts in (sample, solution) order: a solution replaces the best one only if its count exceeds max(best count, 4),
+ * every improvement recomputes the sample budget with RANSACUpdateNumIters(confidence, outlier ratio, 5, budget), and the loop
+ * stops at the budget.
+ *   SFMB200_SAMPLER_SEEDED (default): a counter-based generator (splitmix64 keyed by seed, sample and draw; a repeated index is
+ *   redrawn).  cv:: draws its samples from its own RNG, so the result agrees with cv::findEssentialMat only statistically.
+ *   SFMB200_SAMPLER_OPENCV: cv::findEssentialMat's own samples; seed is ignored.  Checked against cv2 4.13:
+ *     identical: the samples and their order (cv::RNG restarted at (uint64)-1 for every pair, getSubset's redraws of a repeated
+ *     index, no subset check), the per-solution inlier counts as far as the solutions agree, the selection and `iterations`;
+ *     equal to rounding: E, about 1e-12 after sign and scale normalisation on the crazyhorse pairs (up to a few 1e-7 where the
+ *     winning sample is ill-conditioned); hence inlier_mask, R, t and pose_mask;
+ *     could in principle differ: a point whose Sampson error lies within rounding of the threshold; a sample on which the two
+ *     five-point solvers disagree (ill-conditioned), if it would hold the winner; and a tie between two solutions of one sample
+ *     that both improve on the best and decide the final winner: here the solution with the smaller root z wins (ascending
+ *     order), in cv:: the one its polynomial solver lists first.  None of these changes a result on the crazyhorse pairs.
  * The pose is recoverPose's: E = U diag(s, s, 0) V^T, candidates [U W V^T | t], [U W^T V^T | t], [.. | -t], [.. | -t]
  * with t = U[:, 2]; a point counts for a candidate when its DLT triangulation against [I|0] has Q2 Q3 > 0, depth < distance_thresh in
  * the first camera, depth in (0, distance_thresh) in the second and its RANSAC inlier flag set; the first candidate whose count is
@@ -290,15 +300,19 @@ int sfmb200_ransac_score(sfmb200_ctx* ctx, int model, const float* a, const floa
  *   recoverPose's (the pruning mask); either may be NULL.  opt NULL = defaults.  summary may be NULL.
  *   m < 5 or no model: SFMB200_OK with summary.found = 0, E / R / t / masks zero.
  *   m == 5: cv::findEssentialMat returns every solution of the one sample stacked (and the reference's recoverPose would then
- *   fail on the 3n x 3 matrix); here the one sample goes through the same selection as every other call.
- * Same seed, same inputs: bitwise-identical outputs.  One host synchronisation per call.
+ *   fail on the 3n x 3 matrix); here the one sample goes through the same selection as every other call.  Under
+ *   SFMB200_SAMPLER_OPENCV that sample is the five points in their order, as cv:: solves them.
+ *   SFMB200_ERR_INVALID: bad options (including a sampler other than the two below), a NULL K, a zero or non-finite focal length.
+ * Same options, same inputs: bitwise-identical outputs.  One host synchronisation per call.
  */
+enum { SFMB200_SAMPLER_SEEDED = 0, SFMB200_SAMPLER_OPENCV = 1 };
 typedef struct {
     int max_iters;            /* 1000  cv::findEssentialMat default; >= 1 */
     double confidence;        /* 0.999 (SfMStereoUtilities.cpp:97); in (0, 1) */
     double threshold_px;      /* 1.0   (:97); > 0 */
     double distance_thresh;   /* 50    cv::recoverPose default; > 0 */
-    uint64_t seed;            /* 0 */
+    uint64_t seed;            /* 0     SFMB200_SAMPLER_SEEDED only */
+    int sampler;              /* SFMB200_SAMPLER_SEEDED; or SFMB200_SAMPLER_OPENCV */
 } sfmb200_essential_options;
 typedef struct {
     int found;                /* 1: a model with more than 4 inliers */
@@ -325,7 +339,7 @@ int sfmb200_essential_last_trace(sfmb200_ctx* ctx, int cap, int32_t* samples, in
  * match_off, their checks and n_pairs == 0 are described under "image-pair batches" above.  Pair p's outputs
  * (E, R, t, its slices of both masks, summary[p]) are bitwise what sfmb200_find_camera_matrices returns for that pair's matches
  * with the same options, whatever else is in the batch and wherever the pair stands in it: one seed covers the call and every
- * pair draws its samples from it as a single call does.  Per pair as in the single call: m < 5 gives found = 0 and zeros, m == 5
+ * pair draws its samples from it as a single call does (under SFMB200_SAMPLER_OPENCV from its own cv::RNG((uint64)-1)).  Per pair as in the single call: m < 5 gives found = 0 and zeros, m == 5
  * one sample, no model found = 0 with zeros.
  *   K [9] float row-major, shared by all pairs.
  *   E [n_pairs * 9], R [n_pairs * 9], t [n_pairs * 3]: any may be NULL.  inlier_mask / pose_mask [match_off[n_pairs]]: either

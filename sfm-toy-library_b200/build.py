@@ -94,6 +94,22 @@ def build_host_essential(force=False):
     return out
 
 
+def build_host_essential_opencv(force=False):
+    """The shim built with SFMB200_SHIM_ESSENTIAL_OPENCV (findCameraMatricesFromMatch on the device with cv::findEssentialMat's own
+    samples) + its test program, which runs the stage on image pairs read from a file."""
+    hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_essential_opencv")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    deps = [os.path.join(hdir, f) for f in ("shim.cpp", "test_shim_essential_opencv.cpp", "sfmtoylib_b200.h", "sfm_features.h", "cv_min.h")] + [SO]
+    if force or _stale(out, deps):
+        r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", "-DSFMB200_SHIM_ESSENTIAL_OPENCV", os.path.join(hdir, "shim.cpp"),
+                            os.path.join(hdir, "test_shim_essential_opencv.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
+                            "-lpthread", "-o", out], capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("host shim (SFMB200_SHIM_ESSENTIAL_OPENCV) build failed")
+    return out
+
+
 def build_host_homography(force=False):
     """The shim built with SFMB200_SHIM_HOMOGRAPHY (findHomographyInliers on the device too) + its test binary."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_shim_homography")
@@ -190,6 +206,7 @@ if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
     print(build_host(force="--force" in sys.argv))
     print(build_host_essential(force="--force" in sys.argv))
+    print(build_host_essential_opencv(force="--force" in sys.argv))
     print(build_host_homography(force="--force" in sys.argv))
     print(build_host_pose(force="--force" in sys.argv))
     print(build_images(force="--force" in sys.argv))

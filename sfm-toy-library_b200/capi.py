@@ -16,6 +16,7 @@ RATIO_REFERENCE = float(np.float64(np.float32(0.8)))     # NN_MATCH_RATIO = (dou
 MIN_REPROJECTION_ERROR = 10.0                            # SfMStereoUtilities.cpp:42
 CONVERGENCE, NO_CONVERGENCE, FAILURE = 0, 1, 2
 MODEL_HOMOGRAPHY, MODEL_ESSENTIAL, MODEL_POSE = 0, 1, 2
+SAMPLER_SEEDED, SAMPLER_OPENCV = 0, 1                      # sfmb200_essential_options.sampler
 
 _lib = None
 
@@ -50,7 +51,7 @@ class BASummary(C.Structure):
 
 class EssentialOptions(C.Structure):
     _fields_ = [("max_iters", C.c_int), ("confidence", C.c_double), ("threshold_px", C.c_double), ("distance_thresh", C.c_double),
-                ("seed", C.c_uint64)]
+                ("seed", C.c_uint64), ("sampler", C.c_int)]
 
 
 class EssentialSummary(C.Structure):
@@ -285,8 +286,9 @@ class Context:
     # ------------------------------------------------------------------ f-2 essential-matrix RANSAC + pose recovery
     def find_camera_matrices(self, K, pts_left, pts_right, match_q=None, match_t=None, options=None, **kw):
         """sfmb200_find_camera_matrices: findEssentialMat(RANSAC) + recoverPose on the device.  options: EssentialOptions or
-        keyword overrides of the defaults (max_iters, confidence, threshold_px, distance_thresh, seed).
-        Returns (E [3,3], R [3,3], t [3], inlier_mask [m], pose_mask [m], summary dict)."""
+        keyword overrides of the defaults (max_iters, confidence, threshold_px, distance_thresh, seed, sampler).  sampler=SAMPLER_OPENCV
+        draws cv::findEssentialMat's own samples (seed ignored), so E and the masks are OpenCV's; SAMPLER_SEEDED (default) draws
+        seeded ones.  Returns (E [3,3], R [3,3], t [3], inlier_mask [m], pose_mask [m], summary dict)."""
         K = np.ascontiguousarray(K, np.float32).reshape(9)
         L = np.ascontiguousarray(pts_left, np.float32).reshape(-1, 2); R = np.ascontiguousarray(pts_right, np.float32).reshape(-1, 2)
         if match_q is not None:
@@ -304,8 +306,8 @@ class Context:
     def find_camera_matrices_pairs(self, K, points, pairs, match_q, match_t, match_off, options=None, **kw):
         """sfmb200_find_camera_matrices_pairs: find_camera_matrices for every pair in one call, with the arguments of
         find_homography_pairs (points: list of [n_i, 2] key points per image; pairs [P, 2]; match_q / match_t: all pairs' matches
-        concatenated, pair p owning match_off[p]:match_off[p+1]).  options: EssentialOptions or keyword overrides of the defaults.
-        Returns (E [P, 3, 3], R [P, 3, 3], t [P, 3], inlier_mask [sum of matches], pose_mask [sum of matches], summary dict of
+        concatenated, pair p owning match_off[p]:match_off[p+1]).  options: EssentialOptions or keyword overrides of the defaults
+        (sampler as in find_camera_matrices).  Returns (E [P, 3, 3], R [P, 3, 3], t [P, 3], inlier_mask [sum of matches], pose_mask [sum of matches], summary dict of
         arrays found / n_inliers / n_good / iterations / n_samples / n_hypotheses [P])."""
         K = np.ascontiguousarray(K, np.float32).reshape(9)
         batch, P, M = _pair_batch_args(points, pairs, match_q, match_t, match_off)

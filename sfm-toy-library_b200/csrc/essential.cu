@@ -4,10 +4,14 @@
 //   cv::findEssentialMat(RANSAC, 0.999, 1 px) -> cv::recoverPose(E, ..., mask)
 // for every pair of a call (sfmb200_find_camera_matrices_pairs; sfmb200_find_camera_matrices is a call with one pair).  The
 // correspondences of all pairs are concatenated; pair p draws S_p samples (0 for m < 5, 1 for m == 5, else max_iters).  The pairs
-// are cut into consecutive groups whose hypotheses (10 slots of 96 B per sample) fit ES_HYP_BUDGET; per group, three launches:
-//   1. essential_solve_kernel      one thread per sample of the group: draw 5 distinct correspondences of its pair (splitmix64
-//                                  keyed by seed, the sample's index within its pair and draw), normalise them, five-point
-//                                  solver (essential_math.cuh) -> up to 10 E per sample in slot 10 s + k
+// are cut into consecutive groups whose hypotheses (10 slots of 96 B per sample) fit ES_HYP_BUDGET; per group, three launches
+// (four with the OpenCV sampler):
+//   0. essential_cv_sample_kernel  SFMB200_SAMPLER_OPENCV only, one thread per pair of the group: the pair's S samples as
+//                                  cv::findEssentialMat draws them (em_cv_samples: cv::RNG((uint64)-1), getSubset's redraws),
+//                                  serially, since a redraw shifts the rest of the stream
+//   1. essential_solve_kernel      one thread per sample of the group: its 5 distinct correspondences (drawn here with
+//                                  splitmix64 keyed by seed, the sample's index within its pair and draw, or read from launch
+//                                  0), normalised, five-point solver (essential_math.cuh) -> up to 10 E per sample in slot 10 s + k
 //   2. essential_score_kernel      one CTA per sample: every point of the pair is normalised once and tested against all the
 //                                  sample's solutions with the Sampson error and inlier rule of is_inlier<1> (ransac_score.cuh,
 //                                  the arithmetic sfmb200_ransac_score pins against cv2); empty slots score 0
@@ -19,8 +23,8 @@
 //                                  cv::triangulatePoints' algorithm) against the four pose candidates, recoverPose's depth tests,
 //                                  per-pair, per-candidate counts
 //   5. essential_pose_kernel       per pair the first candidate with the largest count (recoverPose's if-chain): R, t, pruning mask
-// One upload, one download, one host synchronisation per call.  A pair's outputs depend on its own matches, the options and the
-// seed only: not on the other pairs of the call, its position or the grouping.
+// One upload, one download, one host synchronisation per call.  A pair's outputs depend on its own matches and the options only:
+// not on the other pairs of the call, its position or the grouping.
 // For a call with one pair the samples, solution counts and per-slot inlier counts stay on the device (ctx->ess_trace) for
 // sfmb200_essential_last_trace.
 #include <algorithm>
@@ -35,6 +39,7 @@ constexpr int ES_SOLVE_THREADS = 32;     // one sample per thread; 1000 samples 
 constexpr int ES_SCORE_THREADS = 128;    // one sample per CTA; the pairs of a run have a few hundred to a few thousand matches
 constexpr int ES_SELECT_WARPS = 4;       // one pair per warp
 constexpr int ES_POINT_THREADS = 128;
+constexpr int ES_CV_SAMPLE_THREADS = 32;  // one pair per thread; a group holds a few hundred pairs at max_iters 1000
 constexpr size_t ES_HYP_BUDGET = size_t(256) << 20;    // device bytes of hypotheses per group of pairs
 
 struct EsPair {
@@ -62,23 +67,37 @@ __device__ __forceinline__ int es_owner(const EsPair* __restrict__ pr, int np, i
     return lo;
 }
 
+// one thread per pair of the group: the pair's samples as cv::findEssentialMat draws them (em_cv_samples), into the group's buffer
+__global__ void __launch_bounds__(ES_CV_SAMPLE_THREADS)
+essential_cv_sample_kernel(const EsPair* __restrict__ pr, int np, int32_t* __restrict__ samples) {
+    const int p = blockIdx.x * ES_CV_SAMPLE_THREADS + threadIdx.x;
+    if (p >= np) return;
+    const EsPair P = pr[p];
+    em_cv_samples(P.m, P.S, samples + 5 * (size_t)P.s0);
+}
+
 __global__ void __launch_bounds__(ES_SOLVE_THREADS)
 essential_solve_kernel(const float* __restrict__ ga, const float* __restrict__ gb, const EsPair* __restrict__ pr, int np, int Sg, uint64_t seed,
-                       double f, double cx, double cy, int32_t* __restrict__ samples, int32_t* __restrict__ nsol, Model* __restrict__ hyp) {
+                       bool drawn, double f, double cx, double cy, int32_t* __restrict__ samples, int32_t* __restrict__ nsol, Model* __restrict__ hyp) {
     const int s = blockIdx.x * ES_SOLVE_THREADS + threadIdx.x;
     if (s >= Sg) return;
     const EsPair P = pr[es_owner<&EsPair::s0>(pr, np, s)];
     const float* a = ga + 2 * P.off;
     const float* b = gb + 2 * P.off;
     int idx[5];
-    em_sample(seed, (uint32_t)(s - P.s0), P.m, idx);
+    if (drawn) {
+#pragma unroll
+        for (int j = 0; j < 5; ++j) idx[j] = samples[5 * s + j];
+    } else {
+        em_sample(seed, (uint32_t)(s - P.s0), P.m, idx);
+    }
     double x1[5][2], x2[5][2];
 #pragma unroll
     for (int j = 0; j < 5; ++j) {
         // cv::findEssentialMat(points, focal, pp): (x - cx) / focal in double, the normalisation is_inlier<1> applies
         x1[j][0] = ((double)a[2 * idx[j]] - cx) / f; x1[j][1] = ((double)a[2 * idx[j] + 1] - cy) / f;
         x2[j][0] = ((double)b[2 * idx[j]] - cx) / f; x2[j][1] = ((double)b[2 * idx[j] + 1] - cy) / f;
-        samples[5 * s + j] = idx[j];
+        if (!drawn) samples[5 * s + j] = idx[j];
     }
     double E[10][9];
     const int c = five_point_solve(x1, x2, E);
@@ -255,6 +274,8 @@ int es_check_options(sfmb200_ctx* ctx, const sfmb200_essential_options& o) {
     if (o.max_iters < 1 || !(o.confidence > 0.0 && o.confidence < 1.0) || !(o.threshold_px > 0.0) || !(o.distance_thresh > 0.0))
         return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "essential options: max_iters >= 1, confidence in (0, 1), threshold_px > 0, distance_thresh > 0");
     if ((size_t)o.max_iters * 10 > (size_t)INT32_MAX / 2) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "max_iters too large");
+    if (o.sampler != SFMB200_SAMPLER_SEEDED && o.sampler != SFMB200_SAMPLER_OPENCV)
+        return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "essential options: sampler must be SFMB200_SAMPLER_SEEDED or SFMB200_SAMPLER_OPENCV");
     return SFMB200_OK;
 }
 
@@ -328,8 +349,13 @@ int es_run(sfmb200_ctx* ctx, const sfmb200_essential_options& o, double focal, d
         const int p0 = groups[g], np = groups[g + 1] - p0;
         const int Sg = pr[p0 + np - 1].s0 + pr[p0 + np - 1].S;
         if (Sg > 0) {
-            essential_solve_kernel<<<ceil_div(Sg, ES_SOLVE_THREADS), ES_SOLVE_THREADS, 0, ctx->stream>>>(d_a, d_b, d_pr + p0, np, Sg, o.seed, focal, cx, cy,
-                                                                                                         d_samples, d_nsol, d_hyp);
+            const bool drawn = o.sampler == SFMB200_SAMPLER_OPENCV;
+            if (drawn) {
+                essential_cv_sample_kernel<<<ceil_div(np, ES_CV_SAMPLE_THREADS), ES_CV_SAMPLE_THREADS, 0, ctx->stream>>>(d_pr + p0, np, d_samples);
+                SFM_LAUNCH_CHECK(ctx);
+            }
+            essential_solve_kernel<<<ceil_div(Sg, ES_SOLVE_THREADS), ES_SOLVE_THREADS, 0, ctx->stream>>>(d_a, d_b, d_pr + p0, np, Sg, o.seed, drawn, focal,
+                                                                                                         cx, cy, d_samples, d_nsol, d_hyp);
             SFM_LAUNCH_CHECK(ctx);
             essential_score_kernel<<<Sg, ES_SCORE_THREADS, 0, ctx->stream>>>(d_a, d_b, d_pr + p0, np, d_hyp, d_nsol, focal, cx, cy, t2, d_counts);
             SFM_LAUNCH_CHECK(ctx);
@@ -373,6 +399,7 @@ extern "C" {
 void sfmb200_essential_default_options(sfmb200_essential_options* opt) {
     if (!opt) return;
     opt->max_iters = 1000; opt->confidence = 0.999; opt->threshold_px = 1.0; opt->distance_thresh = 50.0; opt->seed = 0;
+    opt->sampler = SFMB200_SAMPLER_SEEDED;
 }
 
 int sfmb200_find_camera_matrices(sfmb200_ctx* ctx, const float* K, const float* pts_left, int n_left, const float* pts_right, int n_right,

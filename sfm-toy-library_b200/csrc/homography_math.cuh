@@ -1,6 +1,6 @@
 // homography_math.cuh -- per-sample and per-pair arithmetic of the homography RANSAC (homography.cu), the algorithm of
 // cv::findHomography(RANSAC) in OpenCV 4.x (calib3d fundam.cpp, ptsetreg.cpp, levmarq.cpp):
-//   * cv::RNG, seeded with (uint64)-1 on every call, and getSubset: four indices drawn one after another, an index that
+//   * cv::RNG, seeded with (uint64)-1 on every call, and getSubset (cv_rng.cuh): four indices drawn one after another, an index that
 //     repeats an earlier one redrawn; the quad is rejected (and four new indices drawn) when the last point is collinear with
 //     two earlier ones in either image, or when the four triples disagree in orientation between the images;
 //   * the normalised 4-point / least-squares DLT of HomographyEstimatorCallback::runKernel: 9 x 9 L^T L, the eigenvector of
@@ -14,6 +14,8 @@
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
+
+#include "cv_rng.cuh"
 
 #if defined(__CUDACC__)
 #define HM_HD __host__ __device__ __forceinline__
@@ -31,13 +33,6 @@
 #endif
 
 constexpr int HM_SUBSET_ATTEMPTS = 10000;     // RANSACPointSetRegistrator::run -> getSubset(..., 10000)
-
-// ---- cv::RNG -------------------------------------------------------------------------------------------------------------
-HM_HD uint32_t hm_rng_next(uint64_t& s) {
-    s = (uint64_t)(uint32_t)s * 4164903690ull + (s >> 32);
-    return (uint32_t)s;
-}
-HM_HD int hm_rng_uniform(uint64_t& s, int n) { return (int)(hm_rng_next(s) % (uint32_t)n); }
 
 // ---- subset checks (HomographyEstimatorCallback::checkSubset) -----------------------------------------------------------
 // haveCollinearPoints for the last of four points; p = x0 y0 x1 y1 ...  The differences are float, as in OpenCV.
@@ -75,15 +70,9 @@ HM_HD bool hm_subset_ok(const float* s, const float* d) {
 HM_HD bool hm_draw_subset(uint64_t& s, int n, const float* a, const float* b, int idx[4]) {
     for (int attempt = 0; attempt < HM_SUBSET_ATTEMPTS; ++attempt) {
         float qa[8], qb[8];
+        cv_rng_distinct<4>(s, n, idx);
         for (int i = 0; i < 4; ++i) {
-            int v;
-            for (;;) {
-                v = hm_rng_uniform(s, n);
-                bool dup = false;
-                for (int k = 0; k < i; ++k) dup |= idx[k] == v;
-                if (!dup) break;
-            }
-            idx[i] = v;
+            const int v = idx[i];
             qa[2 * i] = a[2 * v]; qa[2 * i + 1] = a[2 * v + 1];
             qb[2 * i] = b[2 * v]; qb[2 * i + 1] = b[2 * v + 1];
         }

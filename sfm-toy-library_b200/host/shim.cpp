@@ -4,6 +4,11 @@
 //   SfMToyLib/SfMBundleAdjustmentUtils.cpp:99-222
 // leaves SfM.cpp and main.cpp untouched (INTEGRATION.md).  No arithmetic happens here: only flattening of the
 // std::vector / std::map / cv::Mat containers into the plain arrays of the ABI and back.
+#ifdef SFMB200_SHIM_ESSENTIAL_OPENCV   // the device findCameraMatricesFromMatch with cv::findEssentialMat's own samples
+#ifndef SFMB200_SHIM_ESSENTIAL
+#define SFMB200_SHIM_ESSENTIAL
+#endif
+#endif
 #ifdef SFMB200_WITH_REFERENCE_HEADERS
 #include "SfMToyLib/SfM2DFeatureUtilities.h"
 #include "SfMToyLib/SfMStereoUtilities.h"
@@ -132,6 +137,7 @@ bool SfMStereoUtilities::triangulateViews(const Intrinsics& intrinsics, const Im
 
 #ifdef SFMB200_SHIM_ESSENTIAL      // define it to replace findCameraMatricesFromMatch (OpenCV's findEssentialMat + recoverPose) too
 // SfMStereoUtilities.cpp:74-118: essential-matrix RANSAC and pose recovery in one device call (sfmb200_find_camera_matrices).
+// With SFMB200_SHIM_ESSENTIAL_OPENCV the samples are cv::findEssentialMat's, so the pruned matches are the reference's.
 bool SfMStereoUtilities::findCameraMatricesFromMatch(const Intrinsics& intrinsics, const Matching& matches, const Features& featuresLeft,
                                                      const Features& featuresRight, Matching& prunedMatches, cv::Matx34f& Pleft,
                                                      cv::Matx34f& Pright) {
@@ -147,9 +153,14 @@ bool SfMStereoUtilities::findCameraMatricesFromMatch(const Intrinsics& intrinsic
     double R[9], t[3];
     std::vector<uint8_t> pose_mask(m);
     sfmb200_essential_summary summary;
+    sfmb200_essential_options opt;
+    sfmb200_essential_default_options(&opt);
+#ifdef SFMB200_SHIM_ESSENTIAL_OPENCV
+    opt.sampler = SFMB200_SAMPLER_OPENCV;
+#endif
     check(sfmb200_find_camera_matrices(context(), K, reinterpret_cast<const float*>(featuresLeft.points.data()), (int)featuresLeft.points.size(),
                                        reinterpret_cast<const float*>(featuresRight.points.data()), (int)featuresRight.points.size(),
-                                       mq.data(), mt.data(), m, nullptr, nullptr, R, t, nullptr, pose_mask.data(), &summary),
+                                       mq.data(), mt.data(), m, &opt, nullptr, R, t, nullptr, pose_mask.data(), &summary),
           "sfmb200_find_camera_matrices");
     if (!summary.found) {
         std::cerr << "findCameraMatricesFromMatch: no essential matrix with more than 4 inliers among " << m << " matches" << std::endl;

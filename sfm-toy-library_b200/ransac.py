@@ -112,29 +112,33 @@ def findCameraMatricesFromMatch(intrinsics: Intrinsics, matches, left: Features,
     return True, matches[m.reshape(-1) != 0].copy(), Pleft, Pright
 
 
-def findCameraMatricesFromMatch_gpu(intrinsics: Intrinsics, matches, left: Features, right: Features, ctx=None, seed=0):
+def findCameraMatricesFromMatch_gpu(intrinsics: Intrinsics, matches, left: Features, right: Features, ctx=None, seed=0,
+                                    sampler=capi.SAMPLER_SEEDED):
     """SfMStereoUtilities::findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) entirely on the device
-    (sfmb200_find_camera_matrices: five-point samples, scoring, OpenCV's sequential selection, recoverPose).
+    (sfmb200_find_camera_matrices: five-point samples, scoring, OpenCV's sequential selection, recoverPose).  sampler=
+    capi.SAMPLER_OPENCV draws cv::findEssentialMat's own samples, so the pruned matches are the reference's; seed is then unused.
     Returns (success, prunedMatches, Pleft, Pright) like the reference."""
     ctx = ctx or default_context()
     Pleft = np.eye(3, 4, dtype=np.float32)
-    E, R, t, _, pose_mask, s = ctx.find_camera_matrices(intrinsics.K, left.points, right.points, matches["queryIdx"], matches["trainIdx"], seed=seed)
+    E, R, t, _, pose_mask, s = ctx.find_camera_matrices(intrinsics.K, left.points, right.points, matches["queryIdx"], matches["trainIdx"], seed=seed,
+                                                        sampler=sampler)
     if not s["found"]:
         return False, matches[:0].copy(), Pleft, Pleft.copy()
     Pright = np.concatenate([R, t.reshape(3, 1)], 1).astype(np.float32)           # :105-107
     return True, matches[pose_mask != 0].copy(), Pleft, Pright
 
 
-def cameraMatricesManyPairs(intrinsics: Intrinsics, features, pairs, matches, ctx=None, seed=0):
+def cameraMatricesManyPairs(intrinsics: Intrinsics, features, pairs, matches, ctx=None, seed=0, sampler=capi.SAMPLER_SEEDED):
     """findCameraMatricesFromMatch (SfMStereoUtilities.cpp:74-118) for every pair in one device call
     (sfmb200_find_camera_matrices_pairs).  features: per image Features; pairs [(i, j), ...]; matches: per pair a structured array
     with queryIdx / trainIdx.  Returns one (success, prunedMatches, Pleft, Pright) per pair, each exactly what
-    findCameraMatricesFromMatch_gpu returns for that pair with the same seed."""
+    findCameraMatricesFromMatch_gpu returns for that pair with the same seed and sampler."""
     ctx = ctx or default_context()
     if len(pairs) == 0:
         return []
     mq, mt, off = capi.flatten_matches([m["queryIdx"] for m in matches], [m["trainIdx"] for m in matches])
-    _, R, t, _, pose_mask, s =ctx.find_camera_matrices_pairs(intrinsics.K, [f.points for f in features], pairs, mq, mt, off, seed=seed)
+    _, R, t, _, pose_mask, s =ctx.find_camera_matrices_pairs(intrinsics.K, [f.points for f in features], pairs, mq, mt, off, seed=seed,
+                                                             sampler=sampler)
     out = []
     for p, m in enumerate(matches):
         Pleft = np.eye(3, 4, dtype=np.float32)

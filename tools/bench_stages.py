@@ -152,7 +152,7 @@ def card():
     return torch.cuda.get_device_name(0), pl
 
 
-ESSENTIAL_KERNELS = ("essential_solve_kernel", "essential_score_kernel", "essential_select_kernel", "essential_cheirality_kernel",
+ESSENTIAL_KERNELS = ("essential_cv_sample_kernel", "essential_solve_kernel", "essential_score_kernel", "essential_select_kernel", "essential_cheirality_kernel",
                      "essential_pose_kernel")
 
 
@@ -196,7 +196,8 @@ def measure_essential(ctx, reps=20, profile=False):
     cv2.findEssentialMat(RANSAC, 0.999, 1 px) + cv2.recoverPose on one thread and on all threads.  Then, in the same run, the 21
     pairs as 21 single calls and in one sfmb200_find_camera_matrices_pairs call (host clock, median over reps), a seeded synthetic
     50-image set (1225 pairs) in one call, and with profile=True the per-kernel device time of each from torch.profiler in a
-    separate pass."""
+    separate pass.  Last, the two samplers alternated round by round (seeded against OpenCV's samples, sfmb200_essential_options.sampler)
+    on the same three workloads, and their kernel split."""
     import cv2
     from sfm_toy_library_b200 import capi
     g = np.load(os.path.join(ROOT, "tests", "golden", "cfg1_crazyhorse.npz"))
@@ -245,6 +246,7 @@ def measure_essential(ctx, reps=20, profile=False):
     t_syn = timed(synthetic, 5)
     kernels = {"crazyhorse_21_single_calls": essential_kernel_ms(singles), "crazyhorse_21_one_call": essential_kernel_ms(batched),
                "synthetic_1225_one_call": essential_kernel_ms(synthetic)} if profile else "not profiled"
+    samplers = measure_essential_samplers(ctx, K, pairs, (feats, ch_pairs, ch_q, ch_t, ch_off), sy, reps, profile)
     name, pl = card()
     return {"metric": "essential_ransac_pose_ms_per_call", "gpu_median_ms": float(np.median(gpu)), "gpu_max_ms": float(np.max(gpu)),
             "cv2_1thread_median_ms": float(np.median(one)), "cv2_all_threads_median_ms": float(np.median(allt)),
@@ -253,9 +255,46 @@ def measure_essential(ctx, reps=20, profile=False):
             "crazyhorse_21_single_calls_median_ms": float(np.median(t_single)), "crazyhorse_21_one_call_median_ms": float(np.median(t_batch)),
             "crazyhorse_21_speedup_one_call": float(np.median(t_single) / np.median(t_batch)),
             "synthetic_1225_one_call_median_ms": float(np.median(t_syn)), "synthetic_1225_one_call_max_ms": float(np.max(t_syn)),
-            "synthetic_matches": int(sy[4][-1]), "kernel_ms_torch_profiler": kernels,
+            "synthetic_matches": int(sy[4][-1]), "kernel_ms_torch_profiler": kernels, "samplers": samplers,
             "detail": {"gpu_ms": gpu, "cv2_1thread_ms": one, "cv2_all_threads_ms": allt, "crazyhorse_21_single_calls_ms": t_single,
                        "crazyhorse_21_one_call_ms": t_batch, "synthetic_1225_one_call_ms": t_syn}}
+
+
+def measure_essential_samplers(ctx, K, pairs, crazyhorse, synthetic, reps, profile):
+    """The seeded arm (the default sampler) against the opencv arm (cv::findEssentialMat's own samples) in alternating rounds:
+    crazyhorse per call (median over rounds per pair, then over pairs), the 21 pairs in one call, the 1225 synthetic pairs in one call
+    (host clock around synchronised calls, every call warmed up before the rounds); with profile=True each arm's kernel split."""
+    from sfm_toy_library_b200 import capi
+    arms = {"seeded": {}, "opencv": {"sampler": capi.SAMPLER_OPENCV}}
+    work = {"crazyhorse_21_one_call": lambda kw: ctx.find_camera_matrices_pairs(K, *crazyhorse, **kw),
+            "synthetic_1225_one_call": lambda kw: ctx.find_camera_matrices_pairs(K, *synthetic, **kw)}
+    per_pair = {k: [[] for _ in pairs] for k in arms}
+    calls = {k: {w: [] for w in work} for k in arms}
+    for kw in arms.values():                      # warm-up of every shape in both arms
+        for a, b in pairs:
+            ctx.find_camera_matrices(K, a, b, **kw)
+        for fn in work.values():
+            fn(kw)
+
+    def clock(fn):
+        t0 = time.perf_counter(); fn(); return 1e3 * (time.perf_counter() - t0)
+    for _ in range(max(reps // 2, 1)):
+        for k, kw in arms.items():
+            for p, (a, b) in enumerate(pairs):
+                per_pair[k][p].append(clock(lambda: ctx.find_camera_matrices(K, a, b, **kw)))
+            for w, fn in work.items():
+                calls[k][w].append(clock(lambda: fn(kw)))
+    out = {}
+    for k, kw in arms.items():
+        out[k] = {"crazyhorse_per_call_median_ms": float(np.median([np.median(x) for x in per_pair[k]])),
+                  "crazyhorse_per_call_max_ms": float(np.max([np.median(x) for x in per_pair[k]]))}
+        for w in work:
+            out[k][w + "_median_ms"] = float(np.median(calls[k][w])); out[k][w + "_ms"] = calls[k][w]
+        if profile:
+            out[k]["kernel_ms_torch_profiler"] = {
+                "crazyhorse_21_single_calls": essential_kernel_ms(lambda: [ctx.find_camera_matrices(K, a, b, **kw) for a, b in pairs]),
+                **{w: essential_kernel_ms(lambda: fn(kw)) for w, fn in work.items()}}
+    return out
 
 
 def synthetic_homography_set(images=50, seed=0):
