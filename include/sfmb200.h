@@ -229,6 +229,17 @@ int sfmb200_ba_problem_download(sfmb200_ba_problem* prob, double* cams6, double*
  * cost.  Any output may be NULL.  Multi-GPU: summed over ranks. */
 int sfmb200_ba_problem_reduced_system(sfmb200_ba_problem* prob, const sfmb200_ba_options* opt, double radius,
                                       double* S, double* rhs, double* grad_cf, double* cost);
+/* The dense solve of the reduced system keeps its right-hand side (n = 6 nc + 1 doubles, padded to a multiple of 32 plus one) in
+ * the shared memory of one CTA above 469 cameras.  On an H100 (227 KB per block) that allows n <= 29055, i.e. at most 4842
+ * cameras; sfmb200_ba_problem_create refuses larger problems with SFMB200_ERR_UNSUPPORTED and says so in the message. */
+/* test/diagnostic hook: the dense solve of sfmb200_ba_problem_run (chol.cuh) on `count` SPD systems, back to back on ONE set of
+ * buffers (solve number + 1 per system, as in the LM loop).  A [count][n][n] row-major, only the lower triangle read;
+ * b [count][n].  grid: CTAs of the factorisation, 0 = what a BA problem of this n uses, otherwise 1 .. co-resident count
+ * (larger is refused: deadlock freedom rests on it).  backsolve: 0 = a BA problem's choice, 1 = cluster (refused where its
+ * slices do not fit), 2 = one CTA.  x [count][n]; L [count][n][n] lower factor or NULL; fail [count] the raw failure counter:
+ * 0 = every pivot and paired 2x2 minor was a normal positive double, >= 1000 = a wait timed out.  Any n >= 1. */
+int sfmb200_dense_spd_solve(sfmb200_ctx* ctx, int n, int count, const double* A, const double* b, int grid, int backsolve,
+                            double* x, double* L, int32_t* fail);
 
 /* Multi-GPU exchange over PEER MEMORY instead of NCCL: every rank exports the CUDA-IPC handle of its problem's exchange
  * buffer, the host all-gathers the handles (rank order) and every rank attaches them.  From then on the reduced camera

@@ -327,6 +327,19 @@ class Context:
         self._check(lib().sfmb200_five_point(self._h, _p(x1, C.c_double), _p(x2, C.c_double), ns, _p(E, C.c_double), _p(n, C.c_int32)))
         return E[:ns].reshape(ns, 10, 3, 3), n[:ns]
 
+    def dense_spd_solve(self, A, b, grid=0, backsolve=0, want_L=False):
+        """sfmb200_dense_spd_solve: the bundle adjustment's dense Cholesky solve on A [count, n, n] (lower triangle read), b [count, n],
+        back to back on one set of buffers.  Returns (x [count, n], fail [count]) or, with want_L, (x, L [count, n, n], fail)."""
+        A = np.ascontiguousarray(A, np.float64); b = np.ascontiguousarray(b, np.float64)
+        if A.ndim == 2:
+            A = A[None]
+        n = A.shape[-1]
+        A = A.reshape(-1, n, n); cnt = A.shape[0]; b = b.reshape(cnt, n)
+        x = np.zeros((cnt, n)); fail = np.zeros(cnt, np.int32); L = np.zeros((cnt, n, n)) if want_L else None
+        self._check(lib().sfmb200_dense_spd_solve(self._h, n, cnt, _p(A, C.c_double), _p(b, C.c_double), int(grid), int(backsolve),
+                                                  _p(x, C.c_double), _p(L, C.c_double), _p(fail, C.c_int32)))
+        return (x, L, fail) if want_L else (x, fail)
+
     def essential_last_trace(self):
         """sfmb200_essential_last_trace: (samples [S, 5], nsol [S], counts [sum nsol]) of the last find_camera_matrices call."""
         f = lib().sfmb200_essential_last_trace

@@ -1135,6 +1135,67 @@ template <typename K> static int resident_grid(sfmb200_ba_problem* P, int* cache
     return std::max(1, std::min(work_blocks, *cache));
 }
 
+// Opt a kernel in to `bytes` of dynamic shared memory.  The limit is an attribute of the function, shared by every problem of the
+// process, so it is only ever raised: a smaller problem created later must not lower the limit a live larger one launches with.
+template <typename K> static cudaError_t raise_smem_limit(K* kernel, size_t bytes) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, (const void*)kernel);
+    if (e != cudaSuccess || (size_t)a.maxDynamicSharedSizeBytes >= bytes) return e;
+    return cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
+// K4 set-up for an n x n system, shared by sfmb200_ba_problem_create and sfmb200_dense_spd_solve: clears the ready flags and LL
+// lines (epoch 0), sets the factorisation's grid to the co-resident CTA count (deadlock freedom rests on it), picks the back
+// substitution (backsolve: 0 = cluster where its slices fit, else one CTA; 1 = cluster; 2 = one CTA), refuses what it cannot hold
+// and opts the chosen kernel in to its shared memory.  0 or an SFMB200 status with the reason in msg.
+static int chol_setup(sfmb200_ctx* ctx, int n, int backsolve, unsigned* ready, uint4* ll, int* grid, bool* cluster, char* msg, size_t msg_len) {
+    const int npad = ((n + 1) + NB - 1) / NB * NB, nbk = npad / NB;
+    auto cuda = [&](cudaError_t e, const char* what) { snprintf(msg, msg_len, "%s: %s", what, cudaGetErrorString(e)); return SFMB200_ERR_CUDA; };
+    cudaError_t e;
+    if ((e = cudaMemsetAsync(ready, 0, 4 * (size_t)nbk * nbk, ctx->stream)) != cudaSuccess) return cuda(e, "cudaMemsetAsync(ready)");
+    if ((e = cudaMemsetAsync(ll, 0, chol_ll_bytes(nbk), ctx->stream)) != cudaSuccess) return cuda(e, "cudaMemsetAsync(ll)");
+    int per_sm = 0;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_stream_kernel, CS_THREADS, 0)) != cudaSuccess) return cuda(e, "occupancy");
+    if (per_sm < 1) { snprintf(msg, msg_len, "the dense Cholesky kernel cannot be resident on this device"); return SFMB200_ERR_UNSUPPORTED; }
+    *grid = per_sm * ctx->sm_count;
+    // back substitution on a cluster of BS_CLUSTER SMs while its per-CTA slices fit (n <= 2816, 469 cameras), on one CTA above;
+    // the one-CTA kernel keeps y (8 npad bytes) in shared memory: npad <= 29056 (n <= 29055, 4842 cameras) on an H100
+    const size_t cs = chol_backsolve_cluster_smem(n);
+    const bool cluster_fits = cs <= 200 * 1024 && chol_backsolve_cluster_threads(n) <= 512;
+    *cluster = backsolve == 1 || (backsolve == 0 && cluster_fits);
+    if (*cluster) {
+        if (!cluster_fits) { snprintf(msg, msg_len, "n = %d: the cluster back substitution holds at most n = 2816", n); return SFMB200_ERR_UNSUPPORTED; }
+        if ((e = raise_smem_limit(chol_backsolve_cluster_kernel, cs)) != cudaSuccess) return cuda(e, "cudaFuncSetAttribute(chol_backsolve_cluster_kernel)");
+    } else {
+        int optin = 0; cudaFuncAttributes a;
+        if ((e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device)) != cudaSuccess) return cuda(e, "cudaDeviceGetAttribute");
+        if ((e = cudaFuncGetAttributes(&a, (const void*)chol_backsolve_kernel)) != cudaSuccess) return cuda(e, "cudaFuncGetAttributes");
+        const size_t bs = chol_backsolve_smem(npad), limit = (size_t)optin - a.sharedSizeBytes;
+        if (bs > limit) {
+            snprintf(msg, msg_len, "the reduced system (n = %d) exceeds the back substitution's shared memory: at most n = %d (%d cameras) on this device",
+                     n, (int)(limit / 8 / NB * NB) - 1, ((int)(limit / 8 / NB * NB) - 2) / 6);
+            return SFMB200_ERR_UNSUPPORTED;
+        }
+        if (bs > 48 * 1024 && (e = raise_smem_limit(chol_backsolve_kernel, bs)) != cudaSuccess) return cuda(e, "cudaFuncSetAttribute(chol_backsolve_kernel)");
+    }
+    return SFMB200_OK;
+}
+
+// The dense solve of an assembled system (K4): the dataflow factorisation, then the back substitution `cluster` selects, x = the
+// first n unknowns.  The LM loop passes the solve number on the device (epoch_dev), sfmb200_dense_spd_solve as `epoch`.
+static int chol_solve_launch(sfmb200_ctx* ctx, double* A, int npad, int n, int grid, bool cluster, double* dinv, double* Linv, int* fail,
+                             unsigned* ready, uint4* ll, unsigned epoch, const unsigned* epoch_dev, double* x, const int* skip) {
+    const int nbk = npad / NB, ntasks = chol_stream_tasks(nbk);
+    chol_stream_kernel<<<std::min(ntasks, grid), CS_THREADS, 0, ctx->stream>>>(A, npad, n, nbk, ntasks, dinv, fail, ready, ll, epoch, Linv, nullptr, skip, epoch_dev);
+    SFM_LAUNCH_CHECK(ctx);
+    if (cluster) chol_backsolve_cluster_kernel<<<BS_CLUSTER, chol_backsolve_cluster_threads(n), chol_backsolve_cluster_smem(n), ctx->stream>>>(A, Linv, npad, n, x, fail, skip);
+    else chol_backsolve_kernel<<<1, 640, chol_backsolve_smem(npad), ctx->stream>>>(A, Linv, npad, n, x, skip);
+    SFM_LAUNCH_CHECK(ctx);
+    return SFMB200_OK;
+}
+
 template <int G> static int launch_point_pass(sfmb200_ba_problem* P, const BAView& v, double inv_radius) {
     sfmb200_ctx* ctx = P->ctx;
     const int GB = PT_THREADS / G;
@@ -1297,20 +1358,14 @@ static int schur_pass(sfmb200_ba_problem* P, const sfmb200_ba_options* opt, doub
 
 static int dense_solve(sfmb200_ba_problem* P, const sfmb200_ba_options* opt, double radius, bool lm) {
     sfmb200_ctx* ctx = P->ctx;
-    const int npad = P->npad, nbk = npad / NB;
+    const int npad = P->npad;
     const LMState* st = lm ? P->d_state : nullptr;
     const int* skip = lm ? &P->d_state->status : nullptr;
     ba_assemble_kernel<<<dim3(ceil_div(npad, 128), npad), 128, 0, ctx->stream>>>(summed(P, P->Sblk), summed(P, P->Scf), summed(P, P->Sff), summed(P, P->rhs), summed(P, P->dcf), P->nc, npad, 1.0 / radius,
                                                                                  opt->min_lm_diagonal, opt->max_lm_diagonal, P->A, st, P->solve_counter);
     SFM_LAUNCH_CHECK(ctx);
-    const int ntasks = chol_stream_tasks(nbk);
-    chol_stream_kernel<<<std::min(ntasks, P->chol_grid_stream), CS_THREADS, 0, ctx->stream>>>(P->A, npad, P->n, nbk, ntasks, P->dinv, P->fail + 1, P->chol_ready, P->chol_ll,
-                                                                                          0u, P->Linv, nullptr, skip, P->solve_counter);
-    SFM_LAUNCH_CHECK(ctx);
-    if (P->backsolve_cluster) chol_backsolve_cluster_kernel<<<BS_CLUSTER, chol_backsolve_cluster_threads(P->n), chol_backsolve_cluster_smem(P->n), ctx->stream>>>(P->A, P->Linv, npad, P->n, P->y_cf, P->fail + 1, skip);
-    else chol_backsolve_kernel<<<1, 640, chol_backsolve_smem(npad), ctx->stream>>>(P->A, P->Linv, npad, P->n, P->y_cf, skip);
-    SFM_LAUNCH_CHECK(ctx);
-    return SFMB200_OK;
+    return chol_solve_launch(ctx, P->A, npad, P->n, P->chol_grid_stream, P->backsolve_cluster, P->dinv, P->Linv, P->fail + 1, P->chol_ready, P->chol_ll,
+                             0u, P->solve_counter, P->y_cf, skip);
 }
 
 // Host-side check of the flattened problem (CSR offsets monotone from 0 to nobs, cameras in range and strictly ascending
@@ -1457,21 +1512,10 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
     }
     // camera-major copy (device counting sort)
     CRT(cudaMemsetAsync(cnt, 0, sizeof(int) * 2 * (nc + 1), st));
-    {   // dataflow Cholesky: ready flags start at epoch 0; the grid must stay within the co-resident CTA count
-        const int nbk = P->npad / NB;
-        CRT(cudaMemsetAsync(P->chol_ready, 0, 4 * (size_t)nbk * nbk, st));
-        CRT(cudaMemsetAsync(P->chol_ll, 0, chol_ll_bytes(nbk), st));
-        int per_sm = 0;
-        CRT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, chol_stream_kernel, CS_THREADS, 0));
-        if (per_sm < 1) {
-            cudaStreamSynchronize(st); ba_release_buffers(P); delete P;
-            return sfmb200_fail(ctx, SFMB200_ERR_UNSUPPORTED, "the dense Cholesky kernel cannot be resident on this device");
-        }
-        P->chol_grid_stream = per_sm * ctx->sm_count;
-        // back substitution on a cluster of BS_CLUSTER SMs while its per-CTA slices fit (n <= 2816, 469 cameras), on one CTA above
-        const size_t cs = chol_backsolve_cluster_smem(P->n);
-        P->backsolve_cluster = cs <= 200 * 1024 && chol_backsolve_cluster_threads(P->n) <= 512;
-        if (P->backsolve_cluster) CRT(cudaFuncSetAttribute(chol_backsolve_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cs));
+    {   // dataflow Cholesky and back substitution (K4)
+        char msg[160]; msg[0] = 0;
+        const int crc = chol_setup(ctx, P->n, 0, P->chol_ready, P->chol_ll, &P->chol_grid_stream, &P->backsolve_cluster, msg, sizeof msg);
+        if (crc != SFMB200_OK) { cudaStreamSynchronize(st); ba_release_buffers(P); delete P; return sfmb200_fail(ctx, crc, "%s", msg); }
     }
     CRT(cudaMemsetAsync(P->counters, 0, 64, st));
     {   // mode: gather (default: ba_pair_kernel + ba_combine_kernel, deterministic) needs the pair-list fill's per-warp camera counters in shared
@@ -1501,10 +1545,10 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         // geometry of the camera-major kernel: one balanced wave of slices; partial records (slices + cameras)
         const size_t fill_smem = sizeof(int) * (size_t)(2 * PFILL_WARPS + 1) * nc;
         if (smem > 48 * 1024) {
-            CRT(cudaFuncSetAttribute(cm_sort_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            CRT(cudaFuncSetAttribute(cm_sort_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            CRT(raise_smem_limit(cm_sort_kernel<false>, smem));
+            CRT(raise_smem_limit(cm_sort_kernel<true>, smem));
         }
-        if (fill_smem > 48 * 1024) CRT(cudaFuncSetAttribute(pair_fill_sorted_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fill_smem));
+        if (fill_smem > 48 * 1024) CRT(raise_smem_limit(pair_fill_sorted_kernel, fill_smem));
         {
             int per_sm = 0;
             CRT(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_camera_kernel<true, false>, CAM_THREADS, 0));
@@ -1581,11 +1625,10 @@ int sfmb200_ba_problem_create(sfmb200_ctx* ctx, int nc, int np, int nobs, const 
         // (zstage, sred): above 212 cameras that passes the 48 KB a launch gets without opting in
         const size_t tab = sizeof(double) * 18 * (size_t)nc, zstatic = sizeof(double) * (PT_THREADS / 32) * (32 * 18 + 4);
         if (P->backsub_from_z && tab <= 40 * 1024 && tab + zstatic > 48 * 1024) {
-            const int t = (int)tab;
-            CRT(P->G == 4 ? cudaFuncSetAttribute(ba_backsub_z_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
-                : P->G == 8 ? cudaFuncSetAttribute(ba_backsub_z_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
-                : P->G == 16 ? cudaFuncSetAttribute(ba_backsub_z_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t)
-                : cudaFuncSetAttribute(ba_backsub_z_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, t));
+            CRT(P->G == 4 ? raise_smem_limit(ba_backsub_z_kernel<4, true>, tab)
+                : P->G == 8 ? raise_smem_limit(ba_backsub_z_kernel<8, true>, tab)
+                : P->G == 16 ? raise_smem_limit(ba_backsub_z_kernel<16, true>, tab)
+                : raise_smem_limit(ba_backsub_z_kernel<32, true>, tab));
         }
     }
 #undef CRT
@@ -1730,6 +1773,63 @@ int sfmb200_ba_problem_reduced_system(sfmb200_ba_problem* P, const sfmb200_ba_op
     if (rhs) for (int c = 0; c < n; ++c) rhs[c] = hA[(size_t)n * npad + c];
     if (grad_cf) for (int c = 0; c < n; ++c) grad_cf[c] = hg[c] / hs[c];
     if (cost) *cost = 0.5 * hsum[0];
+    return SFMB200_OK;
+}
+
+int sfmb200_dense_spd_solve(sfmb200_ctx* ctx, int n, int count, const double* A, const double* b, int grid, int backsolve,
+                            double* x, double* L, int32_t* fail) {
+    if (!ctx || n < 1 || count < 0 || backsolve < 0 || backsolve > 2 || grid < 0) return SFMB200_ERR_INVALID;
+    if (count == 0) return SFMB200_OK;
+    if (!A || !b || !x || !fail) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "null buffer");
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    SFM_CUDA(ctx, cudaSetDevice(ctx->device));
+    const int npad = ((n + 1) + NB - 1) / NB * NB, nbk = npad / NB;
+    const size_t sys = (size_t)npad * npad;
+    // one upload: the systems in the layout ba_assemble_kernel leaves (row n = b, pad rows identity), upper triangles included
+    std::vector<double> h(sys * count, 0.0);
+    for (int k = 0; k < count; ++k) {
+        double* H = h.data() + sys * k;
+        for (int r = 0; r < n; ++r) memcpy(H + (size_t)r * npad, A + ((size_t)k * n + r) * n, 8 * (size_t)n);
+        memcpy(H + (size_t)n * npad, b + (size_t)k * n, 8 * (size_t)n);
+        for (int r = n + 1; r < npad; ++r) H[(size_t)r * npad + r] = 1.0;
+    }
+    // [A count][x count][fail count] | dinv | Linv | ready | ll: x and fail follow the factors so that one download serves
+    const size_t bytes = Carver::pad(8 * (sys + npad) * count) + Carver::pad(4 * (size_t)count) + Carver::pad(8 * (size_t)npad) +
+                         Carver::pad(8 * (size_t)npad * NB) + Carver::pad(4 * (size_t)nbk * nbk) + Carver::pad(chol_ll_bytes(nbk)) + 1024;
+    SFM_CUDA(ctx, ctx->scratch.reserve(bytes));
+    Carver cv(ctx->scratch.p);
+    double* dA = cv.take<double>((sys + npad) * count); double* dx = dA + sys * count;
+    int* dfail = cv.take<int>(count); double* dinv = cv.take<double>(npad); double* Linv = cv.take<double>((size_t)npad * NB);
+    unsigned* ready = cv.take<unsigned>((size_t)nbk * nbk); uint4* ll = cv.take<uint4>(chol_ll_bytes(nbk) / sizeof(uint4));
+    int ba_grid = 0; bool cluster = false;
+    char msg[160]; msg[0] = 0;
+    const int rc = chol_setup(ctx, n, backsolve, ready, ll, &ba_grid, &cluster, msg, sizeof msg);
+    if (rc != SFMB200_OK) return sfmb200_fail(ctx, rc, "%s", msg);
+    if (grid > ba_grid) return sfmb200_fail(ctx, SFMB200_ERR_INVALID, "grid %d exceeds the %d co-resident CTAs of the factorisation", grid, ba_grid);
+    SFM_CUDA(ctx, cudaMemcpyAsync(dA, h.data(), 8 * sys * count, cudaMemcpyHostToDevice, ctx->stream));
+    SFM_CUDA(ctx, cudaMemsetAsync(dx, 0, 8 * (size_t)npad * count, ctx->stream));
+    SFM_CUDA(ctx, cudaMemsetAsync(dfail, 0, 4 * (size_t)count, ctx->stream));
+    for (int k = 0; k < count; ++k) {       // back to back on one set of flags, LL lines and inverses: solve number k + 1
+        const int r = chol_solve_launch(ctx, dA + sys * k, npad, n, grid ? grid : ba_grid, cluster, dinv, Linv, dfail + k, ready, ll,
+                                        (unsigned)k + 1u, nullptr, dx + (size_t)npad * k, nullptr);
+        if (r) return r;
+    }
+    // one download: the factors too when L is wanted, else x and fail (contiguous: fail follows x after the carver's padding)
+    const size_t xoff = 8 * sys * count, foff = (size_t)((char*)dfail - (char*)dA), base = L ? 0 : xoff;
+    std::vector<char> out(foff + 4 * (size_t)count - base);
+    SFM_CUDA(ctx, cudaMemcpyAsync(out.data(), (char*)dA + base, out.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    SFM_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    const double* hx = (const double*)(out.data() + xoff - base);
+    const int* hf = (const int*)(out.data() + foff - base);
+    for (int k = 0; k < count; ++k) {
+        memcpy(x + (size_t)k * n, hx + (size_t)npad * k, 8 * (size_t)n);
+        fail[k] = hf[k];
+        if (L) {
+            const double* F = (const double*)out.data() + sys * k;
+            for (int r = 0; r < n; ++r)
+                for (int c = 0; c < n; ++c) L[((size_t)k * n + r) * n + c] = c <= r ? F[(size_t)r * npad + c] : 0.0;
+        }
+    }
     return SFMB200_OK;
 }
 

@@ -47,12 +47,17 @@ __device__ __forceinline__ double chol_rsqrt_fast(double d) {
     return fma(p2, q, y);
 }
 // Two consecutive pivots of a 2x2 block [a00 .; a10 a11] from two INDEPENDENT reciprocal square roots.
+// A pivot a00 or minor D2 is accepted when it is a NORMAL positive double below DBL_MAX: rsqrt.approx.ftz flushes a subnormal to
+// zero and returns +inf, which would hand a non-finite factor back with no failure raised (seen at the last pivot of a matrix,
+// where no later pivot turns NaN).  So fail == 0 means every pivot and every paired minor was in [DBL_MIN, DBL_MAX).  An SPD
+// matrix is factored when its pivots lie within about [1e-150, 1e150] (D2 ~ a00 a11 must neither overflow nor go subnormal),
+// as a Jacobi-scaled BA system does; outside that range the solve reports a failure rather than a wrong answer.
 template <bool TAIL>
 __device__ __forceinline__ void chol_pivot_pair(double a00, double a10, double a11, bool pad0, bool pad1, double& inv0, double& inv1, bool& bad) {
     const double D2 = fma(a00, a11, -(a10 * a10));
     const double s1 = chol_rsqrt_fast(a00), s2 = chol_rsqrt_fast(D2);
     const double sq0 = a00 * s1;                               // sqrt(a00)
-    const bool good0 = a00 > 0.0 && a00 < 1.7976931348623157e308, good1 = D2 > 0.0 && D2 < 1.7976931348623157e308;
+    const bool good0 = a00 >= 2.2250738585072014e-308 && a00 < 1.7976931348623157e308, good1 = D2 >= 2.2250738585072014e-308 && D2 < 1.7976931348623157e308;
     if (!TAIL) {
         inv0 = s1; inv1 = s2 * sq0;
         bad = bad || !good0 || !good1;
