@@ -246,7 +246,9 @@ __host__ __device__ inline int chol_stream_tasks(int nbk) { return nbk + (nbk - 
 //   * the factor of a diagonal tile is streamed out in groups of 4 columns while it is being computed: a fifth warp of the
 //     owner CTA copies the finished columns from shared memory to A and to the LL lines below; every solve of that tile
 //     column consumes the groups as they arrive and finishes a fraction of a microsecond after the factorisation instead
-//     of 4.6 us later (the solve keeps pace: 134 ns per pivot against 190 ns);
+//     of 4.6 us later.  A per-group trace later showed the solving task seeing the groups 0.55 us apart while they were
+//     written 0.35 us apart: its loader warp polled one group at a time, one L2 round trip each.  With the loads of three
+//     groups in flight the step per 32 columns went from ~7.0 to ~4.8 us (H100 80GB HBM3, 700 W);
 //   * the rank-32 updates run on the FP64 tensor pipe (mma.sync.m8n8k4.f64, accumulators in fragment layout for the whole
 //     life of the tile, operands from shared memory with a conflict-free 36-double row stride): 40 LDS + 32 DMMA per warp
 //     instead of 288 LDS + 256 DFMA;
@@ -306,11 +308,25 @@ __device__ __forceinline__ void ll_store(uint4* line, double v, unsigned tag) {
     const unsigned lo = (unsigned)__double2loint(v), hi = (unsigned)__double2hiint(v);
     asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" :: "l"(line), "r"(lo), "r"(tag), "r"(hi), "r"(tag) : "memory");
 }
-__device__ __forceinline__ bool ll_try(const uint4* line, unsigned tag, double& v) {
-    unsigned a, b, c, d;
-    asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "l"(line) : "memory");
-    v = __hiloint2double((int)c, (int)a);
-    return b == tag && d == tag;
+// A poll is split into the load (ll_group_issue: this lane's lines of a group -- row `lane` of its 4 columns where that row
+// exists, rows >= 4g, and lanes 0..3 a reciprocal pivot) and the test of the tags (ll_group_ready), so that the loads of several
+// groups can be in flight at once.
+constexpr int LL_AHEAD = 3;
+__device__ __forceinline__ void ll_load(uint4& d, const uint4* line) {
+    asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(d.x), "=r"(d.y), "=r"(d.z), "=r"(d.w) : "l"(line) : "memory");
+}
+__device__ __forceinline__ double ll_value(const uint4& d) { return __hiloint2double((int)d.z, (int)d.x); }
+__device__ __forceinline__ bool ll_tagged(const uint4& d, unsigned tag) { return d.y == tag && d.w == tag; }
+__device__ __forceinline__ void ll_group_issue(uint4 (&d)[5], const uint4* ll, int c, int g, int lane) {
+    const uint4* grp = ll + ((size_t)c * (NB / PANEL_WARPS) + g) * CHOL_LL_GROUP;
+    if (lane >= PANEL_WARPS * g) { ll_load(d[0], grp + lane); ll_load(d[1], grp + NB + lane); ll_load(d[2], grp + 2 * NB + lane); ll_load(d[3], grp + 3 * NB + lane); }
+    if (lane < PANEL_WARPS) ll_load(d[4], grp + 4 * NB + lane);
+}
+__device__ __forceinline__ bool ll_group_ready(const uint4 (&d)[5], int g, int lane, unsigned tag) {
+    bool r = true;
+    if (lane >= PANEL_WARPS * g) r = ll_tagged(d[0], tag) && ll_tagged(d[1], tag) && ll_tagged(d[2], tag) && ll_tagged(d[3], tag);
+    if (lane < PANEL_WARPS) r = r && ll_tagged(d[4], tag);
+    return r;
 }
 
 // `skip` (every kernel of this file, optional): when it points at a non-zero word the launch is a no-op -- the device-resident
@@ -420,34 +436,33 @@ __global__ void __launch_bounds__(CS_THREADS) chol_stream_kernel(double* __restr
                 }
                 CHOL_TRACE(3);
             } else {
-                // the fifth warp is the loader: it polls the LL lines of the groups in order, running ahead of the solve (the L2
-                // round trip of a poll stays off the chain), and hands group g over with the group's named barrier (ids 2..9)
+                // the fifth warp is the loader: it polls the LL lines of the groups in order and hands group g over with the group's
+                // named barrier (ids 2..9).  The loads of the next LL_AHEAD groups are in flight while a group is handed over, so
+                // that groups already written arrive one L2 round trip apart in total, not one round trip each.
                 bool ok = true;
-#pragma unroll 1
+                uint4 q[LL_AHEAD][5];
+#pragma unroll
+                for (int g = 0; g < LL_AHEAD; ++g) ll_group_issue(q[g], ll, c, g, lane);
+#pragma unroll
                 for (int g = 0; g < NB / PANEL_WARPS; ++g) {
                     const int j0 = PANEL_WARPS * g;
-                    {
-                        // poll this thread's lines of group g: row `lane` of the 4 columns (rows >= 4g exist), lanes 0..3 a reciprocal pivot
-                        const uint4* grp = ll + ((size_t)c * (NB / PANEL_WARPS) + g) * CHOL_LL_GROUP;
-                        const bool has_row = lane >= j0;
-                        double v0 = 0, v1 = 0, v2 = 0, v3 = 0, vi = 0;
-                        bool done = false;
+                    uint4 (&d)[5] = q[g % LL_AHEAD];
+                    if (!ll_group_ready(d, g, lane, epoch)) {
                         const long long t0 = clock64();
                         for (;;) {
-                            bool r = true;
-                            if (has_row) { r = ll_try(grp + lane, epoch, v0); r = ll_try(grp + NB + lane, epoch, v1) && r; r = ll_try(grp + 2 * NB + lane, epoch, v2) && r; r = ll_try(grp + 3 * NB + lane, epoch, v3) && r; }
-                            if (lane < PANEL_WARPS) r = ll_try(grp + 4 * NB + lane, epoch, vi) && r;
-                            if (r) { done = true; break; }
-                            if (clock64() - t0 > CF_TIMEOUT_CYCLES) break;
+                            ll_group_issue(d, ll, c, g, lane);
+                            if (ll_group_ready(d, g, lane, epoch)) break;
+                            if (clock64() - t0 > CF_TIMEOUT_CYCLES) { ok = false; break; }
                         }
-                        ok = done && ok;
-                        __syncwarp();
-                        if (g == 0) CHOL_TRACE_W4(2);
-                        if (has_row) { Ls[lane][j0] = v0; Ls[lane][j0 + 1] = v1; Ls[lane][j0 + 2] = v2; Ls[lane][j0 + 3] = v3; }
-                        if (lane < PANEL_WARPS) invd[j0 + lane] = vi;
                     }
-                    __threadfence_block();
+                    __syncwarp();
+                    if (g == 0) CHOL_TRACE_W4(2);
+                    if (lane >= j0) { Ls[lane][j0] = ll_value(d[0]); Ls[lane][j0 + 1] = ll_value(d[1]); Ls[lane][j0 + 2] = ll_value(d[2]); Ls[lane][j0 + 3] = ll_value(d[3]); }
+                    if (lane < PANEL_WARPS) invd[j0 + lane] = ll_value(d[4]);
+                    // no fence before the arrive: it would wait for the loads in flight; bar.arrive synchronizes with the bar.sync
+                    // of the same barrier (PTX memory model), which orders the shared-memory stores above for the solving warps
                     asm volatile("bar.arrive %0, %1;" ::"r"(2 + g), "n"(CS_THREADS) : "memory");
+                    if (g + LL_AHEAD < NB / PANEL_WARPS) ll_group_issue(d, ll, c, g + LL_AHEAD, lane);
                 }
                 if (!ok) abort_flag = 1;
             }

@@ -2,7 +2,9 @@
 // reduced-camera-system size, checked against a host factorisation, with the critical-path timeline from its %globaltimer
 // trace; then the cluster and the single-CTA back-solves on its factor, checked against a host solve.
 // Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -o tools/_build/chol_microbench tools/chol_microbench.cu
-// Usage: chol_microbench [cams=100] [reps=20]
+// Usage: chol_microbench [cams=100] [reps=20] [flush_mb=0]
+// flush_mb > 0 writes that many MB of scratch before every factorisation, so that its buffers start out of L2 as they do inside
+// an LM iteration, whose passes stream far more than the L2 holds.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -22,7 +24,7 @@ static void decode(int t, int nbk, int& i, int& c, bool& merged) {
 }
 
 int main(int argc, char** argv) {
-    const int nc = argc > 1 ? atoi(argv[1]) : 100, reps = argc > 2 ? atoi(argv[2]) : 20;
+    const int nc = argc > 1 ? atoi(argv[1]) : 100, reps = argc > 2 ? atoi(argv[2]) : 20, flush_mb = argc > 3 ? atoi(argv[3]) : 0;
     const int n = 6 * nc + 1, npad = ((n + 1) + NB - 1) / NB * NB, nbk = npad / NB;
     std::vector<double> A((size_t)npad * npad, 0.0), L;
     srand(7);
@@ -48,6 +50,7 @@ int main(int argc, char** argv) {
     CK(cudaMalloc(&dready, 4 * nbk * nbk)); CK(cudaMalloc(&dLinv, 8 * (size_t)npad * NB)); CK(cudaMalloc(&dx, 8 * npad)); CK(cudaMalloc(&dtrace, 64 * (size_t)nbk * nbk));
     CK(cudaMemcpy(dA0, A.data(), bytes, cudaMemcpyHostToDevice)); CK(cudaMemset(dfail, 0, 16)); CK(cudaMemset(dready, 0, 4 * nbk * nbk)); CK(cudaMalloc(&dprogress, chol_ll_bytes(nbk))); CK(cudaMemset(dprogress, 0, chol_ll_bytes(nbk)));
     cudaDeviceProp prop; CK(cudaGetDeviceProperties(&prop, 0));
+    void* dflush = nullptr; if (flush_mb > 0) CK(cudaMalloc(&dflush, (size_t)flush_mb << 20));
     cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
     unsigned epoch = 0;
     std::vector<double> out((size_t)npad * npad);
@@ -60,6 +63,7 @@ int main(int argc, char** argv) {
         for (int rep = 0; rep < reps + 2; ++rep) {
             const bool traced = rep == reps + 1;
             CK(cudaMemcpy(dA, dA0, bytes, cudaMemcpyDeviceToDevice));
+            if (flush_mb > 0) CK(cudaMemset(dflush, rep & 0xff, (size_t)flush_mb << 20));
             if (traced) CK(cudaMemset(dtrace, 0, 64 * (size_t)nbk * nbk));
             CK(cudaDeviceSynchronize());
             CK(cudaEventRecord(e0));
@@ -74,8 +78,8 @@ int main(int argc, char** argv) {
         for (int r = 0; r <= n; ++r) for (int c = 0; c <= std::min(r, n - 1); ++c) {
             err = std::max(err, std::fabs(out[(size_t)r * npad + c] - L[(size_t)r * npad + c])); ref = std::max(ref, std::fabs(L[(size_t)r * npad + c]));
         }
-        printf("{\"variant\": \"%s\", \"cams\": %d, \"n\": %d, \"tile_rows\": %d, \"grid\": %d, \"tasks\": %d, \"avg_us\": %.1f, \"best_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_L\": %.3e, \"fail\": %d}\n",
-               "streaming dataflow (DMMA updates)", nc, n, nbk, grid, ntasks, total / reps * 1e3, best * 1e3, err, ref, fail[0]);
+        printf("{\"variant\": \"%s\", \"flush_mb\": %d, \"cams\": %d, \"n\": %d, \"tile_rows\": %d, \"grid\": %d, \"tasks\": %d, \"avg_us\": %.1f, \"best_us\": %.1f, \"max_abs_err\": %.3e, \"max_abs_L\": %.3e, \"fail\": %d}\n",
+               "streaming dataflow (DMMA updates)", flush_mb, nc, n, nbk, grid, ntasks, total / reps * 1e3, best * 1e3, err, ref, fail[0]);
         CK(cudaMemcpy(tr.data(), dtrace, 64 * (size_t)ntasks, cudaMemcpyDeviceToHost));
         // critical path: per diagonal tile j, the stamps of the task that factors it
         unsigned long long t_start = ~0ull;
