@@ -629,6 +629,61 @@ int sfmb200_decode_images_extract_orb(sfmb200_ctx* ctx, const uint8_t* const* da
                                       uint8_t* const* out_bgr /* NULL: images not downloaded */, const size_t* out_stride);
 int sfmb200_png_last_stats(const sfmb200_ctx* ctx, int64_t* stats /* [SFMB200_PNG_STATS] */);
 
+/* ---- f-1 on the device: find2D3DMatches and mergeNewPointCloud ------------------------------------------------- */
+/*
+ * The host code between the stages of SfM::addMoreViewsToReconstruction (SfM.cpp:366-469): find2D3DMatches (:471-528) once per added
+ * view and mergeNewPointCloud (:530-600) once per good view, with the results of host/sfm_glue.cpp (which are the reference's).
+ *
+ * The match matrix lives on the device as a match index.  sfmb200_match_index_create takes the image-pair batch layout without pts
+ * (img_off / pairs / match_q / match_t / match_off, the checks of "image-pair batches" above) plus match_d [M], the float distances.
+ * The matrix is upper-triangular: every pair must have left < right and appear at most once (SFMB200_ERR_INVALID otherwise); a pair
+ * absent from the batch has an empty list, and so has the diagonal: a lookup of a view against itself finds nothing.  At most 1024
+ * images, at most INT32_MAX / 4 matches per call.  sfmb200_match_index_set_pair replaces the list of one pair (left < right), as the
+ * driver does at SfM.cpp:288 and :431; every later result is that of an index created from the updated matrix.  Destroy an index
+ * before its context.  Errors of the three calls below are read with sfmb200_last_error(index's context).
+ *
+ * A cloud is given as a view list per point: view_off [n + 1] (from 0, monotone), then view_img / view_feat [view_off[n]], the
+ * (view, feature) pairs of originatingViews in ascending view order.  A view outside [0, n_img), views not strictly ascending, or a
+ * feature outside its view's key points (img_off of the index) is SFMB200_ERR_INVALID with a message; the context stays usable.
+ *
+ * sfmb200_find_2d3d_matches: for every view v with done[v] == 0, in ascending order, the cloud points that hit v: a point hits at its
+ * first originating view (ascending) whose lookup succeeds; for an originating view left of v the first match in list order with
+ * queryIdx == its feature, for one right of v the first with trainIdx == its feature, and the hit's feature in v is that match's
+ * other index.  out_point / out_feat: cloud index and feature index of every hit, view by view and in cloud order inside a view;
+ * view v owns [out_off[v], out_off[v + 1]) (empty for a done view).  The output never exceeds (not-done views) x n_points entries;
+ * if out_cap is below out_off[n_img], the call returns SFMB200_ERR_INVALID with out_off filled and nothing else written.
+ *
+ * sfmb200_merge_point_cloud: mergeNewPointCloud(new points, existing cloud).  Coordinates X [n * 3] float.  Outputs:
+ *   outcome [n_new]  SFMB200_MERGE_APPENDED, _MERGED or _DROPPED per new point (in order);
+ *   target [n_new]   appended: its index in the merged cloud (n_exist + its rank among the appended points); merged: the cloud index
+ *                    of the point the loop broke at (an existing point or an appended one); dropped: -1;
+ *   log_* [log_cap]  every `existingPoint.originatingViews[newKv.first] = newKv.second` of the loop, in the order it runs:
+ *                    log_target (cloud index), log_view / log_feat (the key and value written; an overwrite of an existing key and a
+ *                    key inserted while the same map is iterated are both logged), log_other (the existing key the match confirmed),
+ *                    log_pos (its position in the list of pair (min(view, other), max(view, other)): the debug mergeMatchMatrix entry of
+ *                    :571).  log_other / log_pos may be NULL.
+ *   counts [3]       appended, merged, log entries.
+ * The merged cloud is the existing one, then the appended points in order; applying the log in order to it gives the final maps.
+ * The log never has more than n_img x new_off[n_new] entries (each view of a new point against at most n_img keys of one map); if
+ * log_cap is below counts[2], the call returns SFMB200_ERR_INVALID with counts filled and nothing else written.
+ * Each of the three calls makes one host synchronisation (create and set_pair one more when the index grows); same inputs give
+ * bitwise-identical outputs.
+ */
+typedef struct sfmb200_match_index sfmb200_match_index;
+enum { SFMB200_MERGE_DROPPED = 0, SFMB200_MERGE_APPENDED = 1, SFMB200_MERGE_MERGED = 2 };
+int sfmb200_match_index_create(sfmb200_ctx* ctx, const int32_t* img_off, int n_img, const int32_t* pairs, int n_pairs, const int32_t* match_q,
+                               const int32_t* match_t, const float* match_d, const int64_t* match_off, sfmb200_match_index** index);
+int sfmb200_match_index_set_pair(sfmb200_match_index* index, int left, int right, const int32_t* match_q, const int32_t* match_t,
+                                 const float* match_d, int64_t m);
+void sfmb200_match_index_destroy(sfmb200_match_index* index);
+int sfmb200_find_2d3d_matches(sfmb200_match_index* index, const uint8_t* done /* [n_img] */, int n_points, const int32_t* view_off,
+                              const int32_t* view_img, const int32_t* view_feat, int64_t out_cap, int32_t* out_point, int32_t* out_feat,
+                              int64_t* out_off /* [n_img + 1] */);
+int sfmb200_merge_point_cloud(sfmb200_match_index* index, int n_exist, const float* X_exist, const int32_t* exist_off, const int32_t* exist_img,
+                              const int32_t* exist_feat, int n_new, const float* X_new, const int32_t* new_off, const int32_t* new_img,
+                              const int32_t* new_feat, int64_t log_cap, int8_t* outcome, int32_t* target, int32_t* log_target,
+                              int32_t* log_view, int32_t* log_feat, int32_t* log_other, int32_t* log_pos, int64_t* counts /* [3] */);
+
 /* ---- multi-GPU plumbing (NCCL, one process per GPU) ------------------------------------------------------ */
 #define SFMB200_UNIQUE_ID_BYTES 128
 int sfmb200_comm_unique_id(uint8_t* id /* [SFMB200_UNIQUE_ID_BYTES] */);       /* rank 0, then broadcast by the host */

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libsfmb200.so")
-SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "pose.cu", "homography.cu", "orb.cu", "decode.cu", "jpeg.cu", "png.cu", "resize.cu"]
+SOURCES = ["ctx.cu", "comm.cu", "match.cu", "match_tc.cu", "triangulate.cu", "ba.cu", "ransac.cu", "essential.cu", "pose.cu", "homography.cu", "orb.cu", "decode.cu", "jpeg.cu", "png.cu", "resize.cu", "glue.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 HOST_CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3",
@@ -188,6 +188,23 @@ def build_glue(force=False):
     return out
 
 
+def build_glue_device(force=False):
+    """DeviceGlue (host/sfm_glue_device.cpp: find2D3DMatches / mergeNewPointCloud over the device glue of libsfmb200) + its test
+    program, which checks it against host/sfm_glue.cpp."""
+    hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_glue_device")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    deps = [os.path.join(hdir, f) for f in ("sfm_glue.cpp", "sfm_glue_device.cpp", "sfm_glue.h", "test_glue_device.cpp", "sfmtoylib_b200.h",
+                                            "cv_min.h")] + [SO]
+    if force or _stale(out, deps):
+        r = subprocess.run([HOST_CXX, "-std=c++17", "-O2", "-Wall", os.path.join(hdir, "sfm_glue.cpp"), os.path.join(hdir, "sfm_glue_device.cpp"),
+                            os.path.join(hdir, "test_glue_device.cpp"), "-I", hdir, "-L", LIBDIR, "-lsfmb200", "-Wl,-rpath,$ORIGIN/../../lib",
+                            "-lpthread", "-o", out], capture_output=True, text=True)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("device glue build failed")
+    return out
+
+
 def build_ply(force=False):
     """ASCII PLY writers of SURVEY.md 8(f-4) (host/sfm_ply.cpp) + the small driver the CPU test feeds scenes to."""
     hdir = os.path.join(HERE, "host"); out = os.path.join(hdir, "build", "test_ply")
@@ -212,4 +229,5 @@ if __name__ == "__main__":
     print(build_images(force="--force" in sys.argv))
     print(build_images_features(force="--force" in sys.argv))
     print(build_glue(force="--force" in sys.argv))
+    print(build_glue_device(force="--force" in sys.argv))
     print(build_ply(force="--force" in sys.argv))

@@ -97,7 +97,7 @@ def lib():
         L.sfmb200_stream.argtypes = [C.c_void_p]
         L.sfmb200_kernel_launches.restype = C.c_int64
         L.sfmb200_kernel_launches.argtypes = [C.c_void_p]
-        for name in ("sfmb200_destroy", "sfmb200_descset_destroy", "sfmb200_ba_problem_destroy"):
+        for name in ("sfmb200_destroy", "sfmb200_descset_destroy", "sfmb200_ba_problem_destroy", "sfmb200_match_index_destroy"):
             getattr(L, name).restype = None
             getattr(L, name).argtypes = [C.c_void_p]
         _lib = L
@@ -575,6 +575,11 @@ class Context:
         return dict(zip(("subsequences", "codewords_first_pass", "codewords_sync", "rounds", "swept", "upload_bytes", "download_bytes"), s.tolist()))
 
     # ------------------------------------------------------------------ multi-GPU
+    # ------------------------------------------------------------------ f-1 glue on the device
+    def match_index(self, n_points, pairs, match_q, match_t, match_d, match_off):
+        """sfmb200_match_index_create: a device-resident match matrix (see MatchIndex)."""
+        return MatchIndex(self, n_points, pairs, match_q, match_t, match_d, match_off)
+
     def comm_init(self, unique_id, rank, nranks):
         buf = (C.c_uint8 * UNIQUE_ID_BYTES).from_buffer_copy(bytes(unique_id)) if unique_id is not None else None
         self._check(lib().sfmb200_comm_init(self._h, buf, int(rank), int(nranks)))
@@ -846,3 +851,94 @@ class BAProblem:
         self.ctx._check(lib().sfmb200_ba_problem_reduced_system(self._h, C.byref(o), C.c_double(radius), _p(S, C.c_double),
                                                                 _p(rhs, C.c_double), _p(g, C.c_double), C.byref(cost)))
         return dict(S=S, rhs=rhs, grad_cf=g, cost=cost.value)
+
+
+MERGE_DROPPED, MERGE_APPENDED, MERGE_MERGED = 0, 1, 2      # sfmb200_merge_point_cloud outcomes
+
+
+def flatten_views(view_maps):
+    """Per point a {view: feature} map -> (view_off int32 [n + 1], view_img, view_feat int32), views ascending inside a point."""
+    off = np.zeros(len(view_maps) + 1, np.int32)
+    img, feat = [], []
+    for i, m in enumerate(view_maps):
+        for v in sorted(m):
+            img.append(v); feat.append(m[v])
+        off[i + 1] = len(img)
+    return off, np.asarray(img, np.int32), np.asarray(feat, np.int32)
+
+
+class MatchIndex:
+    """sfmb200_match_index: the upper-triangular match matrix on the device.  n_points: key points per image; pairs [P, 2] with
+    left < right, each at most once; match_q / match_t / match_d: all pairs' matches concatenated, pair p owning
+    match_off[p]:match_off[p+1].  Absent pairs and the diagonal have empty lists."""
+
+    def __init__(self, ctx, n_points, pairs, match_q, match_t, match_d, match_off):
+        self._ctx = ctx
+        self._h = C.c_void_p()
+        self.n_img = len(n_points)
+        img_off = np.zeros(self.n_img + 1, np.int32); img_off[1:] = np.cumsum(np.asarray(n_points, np.int64))
+        pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
+        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32)
+        md = np.ascontiguousarray(match_d, np.float32); moff = np.ascontiguousarray(match_off, np.int64)
+        ctx._check(lib().sfmb200_match_index_create(ctx._h, _p(img_off, C.c_int32), self.n_img, _p(pairs, C.c_int32), pairs.shape[0],
+                                                    _p(mq, C.c_int32), _p(mt, C.c_int32), _p(md, C.c_float), _p(moff, C.c_int64),
+                                                    C.byref(self._h)))
+        ctx._adopt(self)
+
+    def close(self):
+        if self._h:
+            lib().sfmb200_match_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_pair(self, left, right, match_q, match_t, match_d):
+        """sfmb200_match_index_set_pair: replace the list of pair (left, right)."""
+        mq = np.ascontiguousarray(match_q, np.int32); mt = np.ascontiguousarray(match_t, np.int32); md = np.ascontiguousarray(match_d, np.float32)
+        self._ctx._check(lib().sfmb200_match_index_set_pair(self._h, int(left), int(right), _p(mq, C.c_int32), _p(mt, C.c_int32),
+                                                            _p(md, C.c_float), C.c_int64(mq.shape[0])))
+
+    def find_2d3d_matches(self, done, view_off, view_img, view_feat, capacity=None):
+        """sfmb200_find_2d3d_matches -> (point [H], feat [H], off [n_img + 1]): view v's hits are [off[v], off[v + 1])."""
+        done = np.ascontiguousarray(done, np.uint8)
+        off = np.ascontiguousarray(view_off, np.int32); img = np.ascontiguousarray(view_img, np.int32); feat = np.ascontiguousarray(view_feat, np.int32)
+        n = off.shape[0] - 1
+        cap = int(capacity) if capacity is not None else max(1024, n * 4)
+        out_off = np.zeros(self.n_img + 1, np.int64)
+        for attempt in range(2):
+            op = np.empty(max(cap, 1), np.int32); of = np.empty(max(cap, 1), np.int32)
+            rc = lib().sfmb200_find_2d3d_matches(self._h, _p(done, C.c_uint8), n, _p(off, C.c_int32), _p(img, C.c_int32), _p(feat, C.c_int32),
+                                                 C.c_int64(cap), _p(op, C.c_int32), _p(of, C.c_int32), _p(out_off, C.c_int64))
+            if rc == 1 and attempt == 0 and out_off[-1] > cap:
+                cap = int(out_off[-1])
+                continue
+            self._ctx._check(rc)
+            break
+        return op[:out_off[-1]], of[:out_off[-1]], out_off
+
+    def merge_point_cloud(self, X_exist, exist_views, X_new, new_views, log_capacity=None):
+        """sfmb200_merge_point_cloud.  exist_views / new_views: (view_off, view_img, view_feat) as flatten_views returns them.
+        Returns a dict: outcome [n_new] (MERGE_*), target [n_new], the log (log_target, log_view, log_feat, log_other, log_pos) and
+        counts (appended, merged, log entries)."""
+        Xe = np.ascontiguousarray(X_exist, np.float32).reshape(-1, 3); Xn = np.ascontiguousarray(X_new, np.float32).reshape(-1, 3)
+        ev = [np.ascontiguousarray(a, np.int32) for a in exist_views]; nv = [np.ascontiguousarray(a, np.int32) for a in new_views]
+        ne, nn = Xe.shape[0], Xn.shape[0]
+        cap = int(log_capacity) if log_capacity is not None else max(1024, 4 * int(nv[0][-1]))
+        outcome = np.empty(max(nn, 1), np.int8); target = np.empty(max(nn, 1), np.int32); counts = np.zeros(3, np.int64)
+        for attempt in range(2):
+            log = [np.empty(max(cap, 1), np.int32) for _ in range(5)]
+            rc = lib().sfmb200_merge_point_cloud(self._h, ne, _p(Xe, C.c_float), *[_p(a, C.c_int32) for a in ev], nn, _p(Xn, C.c_float),
+                                                 *[_p(a, C.c_int32) for a in nv], C.c_int64(cap), _p(outcome, C.c_int8), _p(target, C.c_int32),
+                                                 *[_p(a, C.c_int32) for a in log], _p(counts, C.c_int64))
+            if rc == 1 and attempt == 0 and counts[2] > cap:
+                cap = int(counts[2])
+                continue
+            self._ctx._check(rc)
+            break
+        k = int(counts[2])
+        return {"outcome": outcome[:nn], "target": target[:nn], "log_target": log[0][:k], "log_view": log[1][:k], "log_feat": log[2][:k],
+                "log_other": log[3][:k], "log_pos": log[4][:k], "counts": counts}

@@ -21,6 +21,9 @@
 #include <unordered_map>
 #include <vector>
 
+struct sfmb200_ctx;
+struct sfmb200_match_index;
+
 namespace sfmtoylib {
 
 typedef std::vector<std::vector<Matching>> MatchMatrix;                      // SfM.h:50 (upper triangular: [left][right], left < right)
@@ -64,5 +67,27 @@ struct MergeCounts { size_t newPoints = 0, mergedPoints = 0; };
 // when non-null and already sized numImages x numImages.
 MergeCounts mergeNewPointCloud(const PointCloud& cloud, PointCloud& reconstructionCloud, const MatchMatrix& featureMatchMatrix,
                                const MatchIndex& index, MatchMatrix* mergeMatchMatrix = nullptr);
+
+// The same two functions on the GPU (host/sfm_glue_device.cpp over sfmb200_find_2d3d_matches / sfmb200_merge_point_cloud, linked
+// with libsfmb200), with identical results.  The match index lives on the device: construct it after createFeatureMatchMatrix()
+// and call setPair wherever the driver replaces a list (SfM.cpp:288, :431), since the index holds positions into the lists.
+// Every call flattens the clouds once and applies the outcome; a failed call throws std::runtime_error with the library's message.
+class DeviceGlue {
+public:
+    DeviceGlue(sfmb200_ctx* ctx, const std::vector<Features>& imageFeatures, const MatchMatrix& featureMatchMatrix);
+    ~DeviceGlue();
+    DeviceGlue(const DeviceGlue&) = delete;
+    DeviceGlue& operator=(const DeviceGlue&) = delete;
+    void setPair(int left, int right, const Matching& matches);
+    Images2D3DMatches find2D3DMatches(size_t numImages, const std::set<int>& doneViews, const std::vector<Features>& imageFeatures,
+                                      const PointCloud& reconstructionCloud);
+    MergeCounts mergeNewPointCloud(const PointCloud& cloud, PointCloud& reconstructionCloud, const MatchMatrix& featureMatchMatrix,
+                                   MatchMatrix* mergeMatchMatrix = nullptr);
+private:
+    sfmb200_ctx* ctx_;
+    sfmb200_match_index* index_ = nullptr;
+    int numImages_;
+    std::vector<int32_t> hitPoint_, hitFeat_, logTarget_, logView_, logFeat_, logOther_, logPos_;   // reused, grown on demand
+};
 
 }  // namespace sfmtoylib

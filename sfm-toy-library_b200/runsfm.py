@@ -94,7 +94,8 @@ class SfM:
                  adjustBundle: Callable = None, matchAllPairs: Callable = None, findHomographyInliers: Callable = None,
                  findCameraMatricesFromMatch: Callable = None, findCameraPoseFrom2D3DMatch: Callable = None,
                  homographyInliersAllPairs: Callable = None, findCameraMatricesManyPairs: Callable = None,
-                 triangulateManyPairs: Callable = None, trace: Optional[list] = None, verbose: bool = False):
+                 triangulateManyPairs: Callable = None, find2D3DMatches: Callable = None, mergeNewPointCloud: Callable = None,
+                 trace: Optional[list] = None, verbose: bool = False):
         self.mImageFeatures = features
         self.n = len(features)
         w, h = image_size
@@ -114,6 +115,10 @@ class SfM:
         self.findCameraMatricesManyPairs = findCameraMatricesManyPairs
         self.triangulateManyPairs = triangulateManyPairs
         self.findCameraPoseFrom2D3DMatch = findCameraPoseFrom2D3DMatch or findCameraPoseFrom2D3DMatch_cv2
+        # the glue between the stages: injected as find2D3DMatches(numImages, doneViews, matchMatrix, features, cloud) and
+        # mergeNewPointCloud(cloud, reconstructionCloud, matchMatrix, features) (stages.py runs both on the device); default: the loops below
+        self.find2D3DMatchesStage = find2D3DMatches
+        self.mergeNewPointCloudStage = mergeNewPointCloud
         self.trace = trace
         self.verbose = verbose
         self.seconds = {"match": 0.0, "homography": 0.0, "essential": 0.0, "triangulate": 0.0, "bundle": 0.0, "pnp": 0.0, "glue": 0.0}
@@ -295,6 +300,9 @@ class SfM:
 
     def find2D3DMatches(self):
         """SfM.cpp:471-528."""
+        if self.find2D3DMatchesStage is not None:
+            return self._timed("glue", self.find2D3DMatchesStage, self.n, self.mDoneViews, self.mFeatureMatchMatrix, self.mImageFeatures,
+                               self.mReconstructionCloud)
         t0 = time.perf_counter()
         index = {}
         out = {}
@@ -324,6 +332,8 @@ class SfM:
 
     def mergeNewPointCloud(self, cloud):
         """SfM.cpp:530-600 (debug visualisation dropped)."""
+        if self.mergeNewPointCloudStage is not None:
+            return self._timed("glue", self.mergeNewPointCloudStage, cloud, self.mReconstructionCloud, self.mFeatureMatchMatrix, self.mImageFeatures)
         t0 = time.perf_counter()
         index = {}
         recon = self.mReconstructionCloud

@@ -269,3 +269,77 @@ def matchAllPairs(features: List[Features], pairs, ctx=None) -> List[np.ndarray]
         m["queryIdx"] = q; m["trainIdx"] = t; m["distance"] = d
         out.append(m)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ f-1: the driver's glue on the device
+class _GlueIndex:
+    """The device match index of the matrix the glue was last called with.  A list replaced in the matrix (SfM.cpp:288, :431 assign a
+    new list object) goes to the device with set_pair before the next call; a new matrix, context or feature count builds a new index."""
+    state = None
+
+    def __init__(self, ctx, matrix, imageFeatures):
+        self.ctx, self.matrix = ctx, matrix
+        self.sizes = tuple(len(f.points) for f in imageFeatures)
+        n = len(imageFeatures)
+        self.lists = [[matrix[i][j] for j in range(n)] for i in range(n)]          # the objects indexed, kept alive for `is`
+        pairs = [(i, j) for i in range(n) for j in range(i + 1, n) if len(matrix[i][j])]
+        lists = [matrix[i][j] for i, j in pairs]
+        off = np.zeros(len(pairs) + 1, np.int64); off[1:] = np.cumsum([len(m) for m in lists])
+        cat = lambda key, dt: np.concatenate([np.asarray(m[key], dt) for m in lists]) if lists else np.zeros(0, dt)
+        self.index = ctx.match_index(self.sizes, np.asarray(pairs, np.int32).reshape(-1, 2), cat("queryIdx", np.int32),
+                                     cat("trainIdx", np.int32), cat("distance", np.float32), off)
+
+    @classmethod
+    def get(cls, ctx, matrix, imageFeatures):
+        st = cls.state
+        if st is None or st.ctx is not ctx or st.matrix is not matrix or st.sizes != tuple(len(f.points) for f in imageFeatures):
+            if st is not None:
+                st.index.close()
+            st = cls.state = cls(ctx, matrix, imageFeatures)
+            return st.index
+        n = len(st.sizes)
+        for i in range(n):
+            for j in range(i + 1, n):
+                m = matrix[i][j]
+                if m is not st.lists[i][j]:
+                    st.index.set_pair(i, j, m["queryIdx"], m["trainIdx"], m["distance"])
+                    st.lists[i][j] = m
+        return st.index
+
+
+def find2D3DMatches(numImages: int, doneViews, featureMatchMatrix, imageFeatures: List[Features], reconstructionCloud: PointCloud, ctx=None):
+    """SfM::find2D3DMatches (SfM.cpp:471-528) on the device (sfmb200_find_2d3d_matches): {view: (points2D [n, 2], points3D [n, 3])}
+    float32 for every view not in doneViews, exactly what runsfm.SfM's own loop returns.  The match index stays on the device between
+    calls."""
+    ctx = ctx or default_context()
+    index = _GlueIndex.get(ctx, featureMatchMatrix, imageFeatures)
+    done = np.zeros(numImages, np.uint8)
+    for v in doneViews:
+        done[v] = 1
+    view_off, view_img, view_feat = capi.flatten_views([p.originatingViews for p in reconstructionCloud])
+    point, feat, off = index.find_2d3d_matches(done, view_off, view_img, view_feat)
+    X = np.array([p.p for p in reconstructionCloud], np.float32).reshape(-1, 3)
+    out = {}
+    for v in range(numImages):
+        if done[v]:
+            continue
+        sl = slice(off[v], off[v + 1])
+        out[v] = (np.asarray(imageFeatures[v].points, np.float32)[feat[sl]].reshape(-1, 2), X[point[sl]].reshape(-1, 3))
+    return out
+
+
+def mergeNewPointCloud(cloud: PointCloud, reconstructionCloud: PointCloud, featureMatchMatrix, imageFeatures: List[Features], ctx=None):
+    """SfM::mergeNewPointCloud (SfM.cpp:530-600) on the device (sfmb200_merge_point_cloud): appends the new points that are near no
+    cloud point to reconstructionCloud (the objects themselves), applies every originatingViews assignment of the reference's loop
+    in order and returns (appended, merged), exactly as runsfm.SfM's own loop does."""
+    ctx = ctx or default_context()
+    index = _GlueIndex.get(ctx, featureMatchMatrix, imageFeatures)
+    Xe = np.array([p.p for p in reconstructionCloud], np.float32).reshape(-1, 3)
+    Xn = np.array([p.p for p in cloud], np.float32).reshape(-1, 3)
+    r = index.merge_point_cloud(Xe, capi.flatten_views([p.originatingViews for p in reconstructionCloud]), Xn,
+                                capi.flatten_views([p.originatingViews for p in cloud]))
+    for i in np.nonzero(r["outcome"] == capi.MERGE_APPENDED)[0]:
+        reconstructionCloud.append(cloud[i])
+    for t, v, f in zip(r["log_target"].tolist(), r["log_view"].tolist(), r["log_feat"].tolist()):
+        reconstructionCloud[t].originatingViews[v] = f
+    return int(r["counts"][0]), int(r["counts"][1])
